@@ -1,4 +1,4 @@
-"""audio_flamingo_b200 -- B200-native (sm_100a) implementation of Audio Flamingo 3's audio->text forward path.
+"""audio_flamingo_b200 -- H100-native (sm_90a) implementation of Audio Flamingo 3's audio->text forward path.
 
 Public surface (mirrors the reference's module roles, SURVEY.md 8-b):
     AudioFlamingo3ForConditionalGeneration, AudioFlamingo3Encoder, AudioFlamingo3MultiModalProjector, Qwen2ForCausalLM

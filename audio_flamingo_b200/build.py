@@ -1,7 +1,7 @@
-"""In-tree nvcc build of libaf3b200.so for sm_100a (cross-compiles without a GPU).
+"""In-tree nvcc build of libaf3b200.so for sm_90a (cross-compiles without a GPU).
 
 The shared library links against cudart only; the TMA descriptor encoder is fetched from the driver at run time
-(cudaGetDriverEntryPoint), so nothing here needs libcuda at build time.  Objects are cached by source mtime.
+(cudaGetDriverEntryPoint), so nothing here needs libcuda at build time.  Objects are cached by source mtime and compiler flags.
 """
 from __future__ import annotations
 
@@ -19,9 +19,8 @@ LIB = PKG_DIR / "libaf3b200.so"
 
 SOURCES = [
     "common.cu",
-    "gemm_tcgen05.cu",
-    "attention_tcgen05.cu",
-    "attention_v2_tcgen05.cu",
+    "gemm_wgmma.cu",
+    "attention_wgmma.cu",
     "decode_attention.cu",
     "elementwise.cu",
     "logmel.cu",
@@ -29,7 +28,7 @@ SOURCES = [
 ]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -52,6 +51,11 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     nvcc = _nvcc()
     BUILD.mkdir(exist_ok=True)
     hm = _headers_mtime()
+    # objects built with other flags (another architecture, say) are never reused: the flags are part of the cache key
+    stamp = BUILD / "flags.txt"
+    flags = " ".join([nvcc, *NVCC_FLAGS])
+    if not stamp.exists() or stamp.read_text() != flags:
+        force = True
     jobs = []
     objs = []
     for src in SOURCES:
@@ -73,6 +77,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             list(ex.map(run, jobs))
     if jobs or not LIB.exists():
         run([nvcc, "-shared", "-cudart", "static", "-o", str(LIB), *map(str, objs)])
+    stamp.write_text(flags)
     return LIB
 
 

@@ -106,7 +106,7 @@ int sm_count() {
     const int dev = current_device() & 127;
     if (n[dev] == 0) {
         cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-        if (n[dev] <= 0) n[dev] = 148;
+        if (n[dev] <= 0) n[dev] = 132;
     }
     return n[dev];
 }

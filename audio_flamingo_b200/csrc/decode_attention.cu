@@ -4,17 +4,17 @@
 // exactly once per step.
 //
 // One CTA = one (sequence, KV head, split) and serves all G = H/Hkv (<= 16) query heads sharing the KV head.  It streams
-// its share of the live 128-key chunks through a 3-stage TMA ring (K and V tiles of 32 KB each, up to 192 KB in flight
+// its share of the live 128-key chunks through a 2-stage TMA ring (K and V tiles of 32 KB each, up to 128 KB in flight
 // per SM) and keeps an online softmax, flash-decoding style.  The problem is transposed so that the 128 keys / 128
-// output dims are the UMMA M dimension and the (padded) 16 query heads are N:
-//     S^T[key, head] = K_tile[key, :] . Q[head, :]          tcgen05.mma 128x16x16 x 8,  A = K tile (K-major, via TMA)
-//     O^T[dim, head] = V_tile^T[dim, key] . P^T[key, head]   tcgen05.mma 128x16x16 x 8,  A = V tile read MN-major
-// so K and V never pass through registers.  Roles: warps 0-7 softmax + accumulation (thread = key lane for S, = output dim lane
-// for O; the heads are split between two warp groups, see the kernel), warp 8 issues the MMAs, warp 9 the TMA loads.  S, P and
-// the per-chunk O are double-buffered so that S_{i+1} = K_{i+1} Q^T and the loads run ahead of softmax_i, and O_i is folded into
-// the register accumulator after softmax_{i+1} has been handed to the tensor core (the chunk's P.V product is then long complete).
-// Measured (round 2): the K/V ring runs far ahead; what bounds the kernel is the softmax warps' serial chain per chunk (~2 us).
-// Splits: the host picks nz = min(chunks(Tmax), SMs / (B*Hkv)) so that B*Hkv*nz CTAs (one per SM, 207 KB of smem) cover
+// output dims are the wgmma M dimension (two m64 halves) and the (padded) 16 query heads are N:
+//     S^T[key, head] = K_tile[key, :] . Q[head, :]          wgmma m64n16k16 x 2 x 8,  A = K tile (K-major, via TMA)
+//     O^T[dim, head] = V_tile^T[dim, key] . P^T[key, head]   wgmma m64n16k16 x 2 x 8,  A = V tile read MN-major
+// so K and V never pass through registers.  Roles: warps 0-7 softmax + accumulation (thread = key row for S, = output dim row
+// for O; the heads are split between two warp groups, see the kernel), warps 8-11 (one warpgroup) issue the MMAs and store
+// the fp32 results to shared memory, warp 12 issues the TMA loads.  S, P and the per-chunk O are double-buffered so that
+// S_{i+1} = K_{i+1} Q^T and the loads run ahead of softmax_i, and O_i is folded into the register accumulator after
+// softmax_{i+1} has been handed to the tensor core.
+// Splits: the host picks nz = min(chunks(Tmax), SMs / (B*Hkv)) so that B*Hkv*nz CTAs (one per SM, ~177 KB of smem) cover
 // the GPU; the live chunk range [start/128, ceil(ctx/128)) of each sequence is divided evenly over the nz splits at run
 // time.  nz == 1 (config 2: 32 x 4 = 128 CTAs) writes the normalised output directly; otherwise every split writes an
 // (unnormalised o, max, sum) partial and the last-arriving split CTA of a (sequence, KV head) merges them (log-sum-exp
@@ -32,38 +32,20 @@ namespace af3 {
 constexpr int DA_CHUNK = 128;    // keys per ring stage
 constexpr int DA_NH = 16;        // query heads per KV head, padded (UMMA N)
 constexpr int DA_NS_MAX = 3;     // K/V ring stages (template parameter NS: 2 or 3)
-constexpr int DA_THREADS = 320;  // warps 0-7: softmax / accumulate (thread = TMEM lane x head group), warp 8: MMA issue, warp 9: TMA
+constexpr int DA_THREADS = 416;  // warps 0-7: softmax / accumulate (thread = row x head group), warps 8-11: wgmma, warp 12: TMA
 constexpr int DA_D = 128;
 constexpr int DA_STAGE = 2 * DA_CHUNK * DA_D * 2;  // K tile + V tile
+constexpr int DA_LD = DA_NH + 1;                   // row pitch (floats) of the S / O result tiles: conflict-free column reads
 constexpr int da_smem(int ns) {
     return ns * DA_STAGE + 2 * (DA_NH * 128) /*Q: 2 blocks of 16 x 128 B*/ + 2 * 2 * (DA_NH * 128) /*P, double-buffered*/ +
-           1024 /*align*/ + 2048 /*barriers + reduction scratch*/;
+           4 * 128 * DA_LD * 4 /*S, O: double-buffered [128][DA_LD] fp32*/ + 1024 /*align*/ + 2048 /*barriers + reduction scratch*/;
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-// 32 lanes x N consecutive columns (N = 4 or 8)
+// N consecutive fp32 columns of one row of an S / O result tile
 template <int N>
-__device__ __forceinline__ void tmem_ldn(uint32_t taddr, uint32_t (&v)[N]) {
-    static_assert(N == 4 || N == 8, "tmem_ldn");
-    if constexpr (N == 4) {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-                     : "r"(taddr)
-                     : "memory");
-    } else {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                     : "r"(taddr)
-                     : "memory");
-    }
+__device__ __forceinline__ void res_ldn(const float* p, uint32_t (&v)[N]) {
+#pragma unroll
+    for (int g = 0; g < N; ++g) v[g] = __float_as_uint(p[g]);
 }
 
 // Merge of the split partials of one (sequence, KV head), executed by the last-arriving split CTA.  Partial layout
@@ -123,11 +105,10 @@ __device__ __forceinline__ float da_exp2(float x) {
 }
 
 // NG = padded query heads per KV head (8 when G <= 8, else 16).  The per-head loops are branch-free so the independent shuffle /
-// SFU chains interleave (ncu r01b: 90 % of the softmax warps' samples sat in those chains).
-// Two warp groups split the heads (round 2): the in-graph timeline showed the kernel bound by the softmax warps' serial work per
-// 128-key chunk (~2 us x 7 chunks at context 800, the K/V ring far ahead), not by the stream.  Warps 0-3 take heads [0, NG/2), warps
-// 4-7 heads [NG/2, NG) of the same keys / output dims (warp w and w + 4 share a TMEM lane quarter): half the instructions per
-// thread and chunk, two warps per scheduler, and the two groups only meet at the P hand-off (each has its own named barrier).
+// SFU chains interleave.
+// Two warp groups split the heads: warps 0-3 take heads [0, NG/2), warps 4-7 heads [NG/2, NG) of the same keys / output dims
+// (warp w and w + 4 read the same rows of S / O): half the instructions per thread and chunk, two warps per scheduler, and the two
+// groups only meet at the P hand-off (each has its own named barrier).
 template <int NG, int DA_NS>
 __global__ void __launch_bounds__(DA_THREADS, 1)
 decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
@@ -148,12 +129,13 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 4 * DA_NH * 128);
     uint64_t *q_full = bars, *k_full = bars + 1, *v_full = k_full + DA_NS_MAX, *kv_empty = v_full + DA_NS_MAX,
              *s_full = kv_empty + DA_NS_MAX, *p_full = s_full + 2, *o_full = p_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
     float* red = reinterpret_cast<float*>(bars) + 256;  // [2 parities][4 warps][16 heads] chunk maxima, then [4][16] sums
+    float* sS = reinterpret_cast<float*>(bars) + 512;   // S^T results [2][128 keys][DA_LD], then O^T results [2][128 dims][DA_LD]
+    float* sO = sS + 2 * 128 * DA_LD;
     __shared__ int last_flag;
 
     // ---- prologue (no global-memory reads: overlaps the tail of the previous kernel under PDL)
-    if (tid == 256) {
+    if (tid == 384) {
         tma_prefetch_desc(&map_q);
         tma_prefetch_desc(&map_k);
         tma_prefetch_desc(&map_v);
@@ -161,25 +143,18 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         for (int s = 0; s < DA_NS; ++s) {
             mbar_init(k_full + s, 1);
             mbar_init(v_full + s, 1);
-            mbar_init(kv_empty + s, 1);
+            mbar_init(kv_empty + s, 4);   // one arrival per wgmma warp
         }
         for (int s = 0; s < 2; ++s) {
-            mbar_init(s_full + s, 1);
+            mbar_init(s_full + s, 128);
             mbar_init(p_full + s, 256);
-            mbar_init(o_full + s, 1);
+            mbar_init(o_full + s, 128);
         }
         fence_barrier_init();
     }
-    if (warp == 0) {
-        tmem_alloc(tmem_slot, 64);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_S = *tmem_slot, tmem_O = tmem_S + 2 * DA_NH;  // S0 S1 O0 O1, 16 columns each
     pdl_launch_dependents();
-    if (l2_prefetch && warp == 9 && lane == 0) {
+    if (l2_prefetch && warp == 12 && lane == 0) {
         // Before the dependency resolves: ask L2 for this CTA's K/V chunks.  Only a hint -- nothing is read into the SM, so it does not
         // matter that ctx_len may still hold the previous step's value or that the row the q/k/v projection is appending right now is
         // not there yet (its write lands in the same L2 line; the real loads below come after griddepcontrol.wait).
@@ -211,7 +186,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     const int n = max(min(c_hi, c_beg + cps) - c_beg, 0);
 
     if (n > 0) {
-        if (warp == 9) {
+        if (warp == 12) {
             if (lane == 0) {
                 mbar_arrive_expect_tx(q_full, 2 * DA_NH * 128);
 #pragma unroll
@@ -230,49 +205,68 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 }
             }
             __syncwarp();
-        } else if (warp == 8) {
-            if (lane == 0) {
-                constexpr uint32_t idesc_s = make_idesc_bf16(128, DA_NH, 0, 0);
-                constexpr uint32_t idesc_o = make_idesc_bf16(128, DA_NH, 1, 0);  // A (= V tile) is MN-major
-                const uint32_t aKV = smem_u32(sKV), aQ = smem_u32(sQ), aP = smem_u32(sP);
-                // O^T_j = V_j^T . P_j^T  (fresh accumulator: the running output lives in registers)
-                auto issue_pv = [&](int j) {
-                    const int s = j % DA_NS;
-                    mbar_wait(p_full + (j & 1), (j >> 1) & 1);
-                    mbar_wait(v_full + s, (j / DA_NS) & 1);
-                    tc_fence_after();
-                    const uint32_t aV = aKV + s * DA_STAGE + 32768, aPj = aP + (j & 1) * (2 * DA_NH * 128);
+        } else if (warp >= 8) {
+            // ---- wgmma warpgroup: each product is two m64 halves (keys / output dims [0, 64) and [64, 128)); the fp32 results
+            //      go to the S / O tiles in shared memory, rows = keys / output dims, columns = heads
+            const int tw = tid - 256;
+            const uint32_t aKV = smem_u32(sKV), aQ = smem_u32(sQ), aP = smem_u32(sP);
+            auto store = [&](float* dst, float (&r)[2][8]) {
+#pragma unroll
+                for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) dst[(mh * 64 + frag_row(tw, e)) * DA_LD + frag_col(tw, e)] = r[mh][e];
+            };
+            // O^T_j = V_j^T . P_j^T  (fresh accumulator: the running output lives in the softmax warps' registers)
+            auto issue_pv = [&](int j) {
+                const int s = j % DA_NS;
+                mbar_wait(p_full + (j & 1), (j >> 1) & 1);
+                mbar_wait(v_full + s, (j / DA_NS) & 1);
+                const uint32_t aV = aKV + s * DA_STAGE + 32768, aPj = aP + (j & 1) * (2 * DA_NH * 128);
+                float r[2][8];
+                wgmma_fence();
+#pragma unroll
+                for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
                     for (int kk = 0; kk < DA_CHUNK / 16; ++kk)
-                        umma_bf16_ss(tmem_O + (j & 1) * DA_NH, make_smem_desc_sw128(aV + kk * 2048, 16384, 1024),
-                                     make_smem_desc_sw128(aPj + (kk >> 2) * (DA_NH * 128) + (kk & 3) * 32, 0, 1024), idesc_o, kk != 0);
-                    umma_commit(o_full + (j & 1));
-                    umma_commit(kv_empty + s);
-                };
-                mbar_wait(q_full, 0);
-                for (int i = 0; i < n; ++i) {
-                    const int s = i % DA_NS;
-                    // S^T_i = K_i . Q^T into S[i & 1]: that buffer was last read by softmax_{i-2}, whose P the previous
-                    // iteration's issue_pv(i - 2) has already waited for
-                    mbar_wait(k_full + s, (i / DA_NS) & 1);
-                    tc_fence_after();
-                    const uint32_t aK = aKV + s * DA_STAGE;
+                        wgmma_m64n16_ss<1, 0>(r[mh], make_smem_desc_sw128(aV + mh * 16384 + kk * 2048, 16384, 1024),
+                                              make_smem_desc_sw128(aPj + (kk >> 2) * (DA_NH * 128) + (kk & 3) * 32, 0, 1024), kk != 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(r[0]);
+                fence_regs(r[1]);
+                if (lane == 0) mbar_arrive(kv_empty + s);
+                store(sO + (j & 1) * 128 * DA_LD, r);
+                mbar_arrive(o_full + (j & 1));
+            };
+            mbar_wait(q_full, 0);
+            for (int i = 0; i < n; ++i) {
+                const int s = i % DA_NS;
+                // S^T_i = K_i . Q^T into S[i & 1]: that buffer was last read by softmax_{i-2}, whose P the previous
+                // iteration's issue_pv(i - 2) has already waited for
+                mbar_wait(k_full + s, (i / DA_NS) & 1);
+                const uint32_t aK = aKV + s * DA_STAGE;
+                float r[2][8];
+                wgmma_fence();
+#pragma unroll
+                for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
                     for (int kk = 0; kk < D / 16; ++kk)
-                        umma_bf16_ss(tmem_S + (i & 1) * DA_NH, make_smem_desc_sw128(aK + (kk >> 2) * 16384 + (kk & 3) * 32, 0, 1024),
-                                     make_smem_desc_sw128(aQ + (kk >> 2) * (DA_NH * 128) + (kk & 3) * 32, 0, 1024), idesc_s, kk != 0);
-                    umma_commit(s_full + (i & 1));
-                    if (i >= 1) issue_pv(i - 1);
-                }
-                issue_pv(n - 1);
+                        wgmma_m64n16_ss<0, 0>(r[mh], make_smem_desc_sw128(aK + mh * 64 * 128 + (kk >> 2) * 16384 + (kk & 3) * 32, 0, 1024),
+                                              make_smem_desc_sw128(aQ + (kk >> 2) * (DA_NH * 128) + (kk & 3) * 32, 0, 1024), kk != 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(r[0]);
+                fence_regs(r[1]);
+                store(sS + (i & 1) * 128 * DA_LD, r);
+                mbar_arrive(s_full + (i & 1));
+                if (i >= 1) issue_pv(i - 1);
             }
-            __syncwarp();
+            issue_pv(n - 1);
         } else {
-            // ---- online softmax: thread = key (TMEM lane) for S, = output dim for O; columns = heads [hg * NH, hg * NH + NH)
+            // ---- online softmax: thread = key (row of S) for S, = output dim for O; columns = heads [hg * NH, hg * NH + NH)
             const int wq = warp & 3, hg = warp >> 2;
             const int kt = wq * 32 + lane;  // key within the chunk / output dim
-            const uint32_t lane_off = static_cast<uint32_t>(wq * 32) << 16;
-            const uint32_t col_off = hg * NH;
+            const int col_off = hg * NH;
             const int bar_id = 1 + hg;      // named barrier of this head group's four warps
             float m_run[NH], m_prev[NH], m_pp[NH], l_thr[NH], acc[NH];
 #pragma unroll
@@ -296,10 +290,8 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             // acc is relative to m_from (the running max at its last update); O_j is relative to m_to
             auto accumulate = [&](int j, const float (&m_from)[NH], const float (&m_to)[NH]) {
                 mbar_wait(o_full + (j & 1), (j >> 1) & 1);
-                tc_fence_after();
                 uint32_t ov[NH];
-                tmem_ldn<NH>(tmem_O + (j & 1) * DA_NH + col_off + lane_off, ov);
-                tmem_ld_wait();
+                res_ldn<NH>(sO + ((j & 1) * 128 + kt) * DA_LD + col_off, ov);
 #pragma unroll
                 for (int g = 0; g < NH; ++g) {
                     const float a = (m_from[g] == -INFINITY) ? 0.f : da_exp2(m_from[g] - m_to[g]);
@@ -311,10 +303,8 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 const bool valid = j >= start && j < ctx;
                 float* redm = red + (i & 1) * 64;
                 mbar_wait(s_full + (i & 1), (i >> 1) & 1);
-                tc_fence_after();
                 uint32_t sv[NH];
-                tmem_ldn<NH>(tmem_S + (i & 1) * DA_NH + col_off + lane_off, sv);
-                tmem_ld_wait();
+                res_ldn<NH>(sS + ((i & 1) * 128 + kt) * DA_LD + col_off, sv);
                 float t[NH], mx[NH];
 #pragma unroll
                 for (int g = 0; g < NH; ++g) {
@@ -350,7 +340,6 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                     *reinterpret_cast<bf16*>(blk + gh * 128 + ((((kc >> 3) ^ (gh & 7)) << 4) | ((kc & 7) << 1))) = __float2bfloat16_rn(p);
                 }
                 fence_proxy_async_smem();
-                tc_fence_before();
                 mbar_arrive(p_full + (i & 1));
                 // fold in the previous chunk's P.V (relative to m_prev = running max after chunk i-1)
                 if (i >= 1) accumulate(i - 1, m_pp, m_prev);
@@ -390,10 +379,8 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             }
         }
     }
-    tc_fence_before();
     if (nz > 1) __threadfence();  // partials visible before this split is counted
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_S, 64);
     if (nz == 1) {
         if (tid == 0) trace_mark(trace, 3);
         return;
@@ -436,13 +423,13 @@ int decode_attention(cudaStream_t stream, const bf16* qkv, const bf16* k_cache, 
     AF3_REQUIRE(ctx_len != nullptr, "decode_attention: ctx_len must be a device pointer");
     AF3_REQUIRE(Hkv <= 65535, "decode_attention: too many KV heads");
     const int nz = pick_splits(B, Hkv, Tmax);
-    // ring depth 3 (192 KB in flight).  A 2-stage ring (so that a few-token GEMM could be co-resident under programmatic dependent
-    // launch) was measured in round 2 and is slower (profiles/r02a_decode_timeline_stages3_3_da2.md).
-    constexpr int ns = 3;
+    // ring depth 2 (128 KB in flight): a third stage does not fit next to the S / O result tiles in 227 KB
+    constexpr int ns = 2;
+    static_assert(da_smem(ns) <= 232448, "shared memory per CTA");
     static DeviceOnce once;
     if (once.first()) {
-        AF3_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<8, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, da_smem(3)));
-        AF3_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<16, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, da_smem(3)));
+        AF3_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<8, ns>, cudaFuncAttributeMaxDynamicSharedMemorySize, da_smem(ns)));
+        AF3_CHECK_CUDA(cudaFuncSetAttribute(decode_attn_kernel<16, ns>, cudaFuncAttributeMaxDynamicSharedMemorySize, da_smem(ns)));
     }
     CUtensorMap mq, mk, mv;
     // q heads as rows of 128: the packed projection row of sequence b holds (H + 2 Hkv) such rows
@@ -455,10 +442,10 @@ int decode_attention(cudaStream_t stream, const bf16* qkv, const bf16* k_cache, 
         return e;
     dim3 grid(B, Hkv, nz);
     int* counters = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(scratch) + partial_bytes(B, H, D, Tmax));
-    auto kern = (H / Hkv <= 8) ? decode_attn_kernel<8, 3> : decode_attn_kernel<16, 3>;
+    auto kern = (H / Hkv <= 8) ? decode_attn_kernel<8, ns> : decode_attn_kernel<16, ns>;
     AF3_CHECK_CUDA(launch_kernel(kern, grid, dim3(DA_THREADS), da_smem(ns), stream, mq, mk, mv, scratch, out, counters, H, Hkv, nz,
                                  ctx_len, kv_start, scale * 1.4426950408889634f, trace_next_slot(),
-                                 [] { const char* e = getenv("AF3_L2_PREFETCH_KV"); return e ? atoi(e) : 1; }()));   // on: -21 us per step in two A/B pairs (profiles/r02n_*)
+                                 [] { const char* e = getenv("AF3_L2_PREFETCH_KV"); return e ? atoi(e) : 1; }()));
     return 0;
 }
 

@@ -323,7 +323,7 @@ int im2col_conv2(cudaStream_t stream, const bf16* in, bf16* cols, int n_win, int
     const int T_out = (T - 1) / 2 + 1;
     const long long total16 = static_cast<long long>(n_win) * T_out * (3 * C / 8);
     if (total16 <= 0) return 0;
-    const int grid = static_cast<int>(((total16 + 255) / 256) < 148ll * 16 ? ((total16 + 255) / 256) : 148ll * 16);
+    const int grid = static_cast<int>(((total16 + 255) / 256) < 132ll * 16 ? ((total16 + 255) / 256) : 132ll * 16);
     im2col_conv2_kernel<<<grid, 256, 0, stream>>>(in, cols, C, T, T_out, total16);
     AF3_CHECK_LAUNCH();
     return 0;
@@ -348,7 +348,7 @@ __global__ void pack_gate_up_kernel(const bf16* __restrict__ gate, const bf16* _
 int pack_gate_up(cudaStream_t stream, const bf16* gate, const bf16* up, bf16* packed, int F, int K) {
     AF3_REQUIRE(K % 8 == 0, "pack_gate_up: K must be a multiple of 8");
     const long long total16 = 2ll * ceil_div(F, 128) * 128 * (K / 8);
-    const int grid = static_cast<int>(((total16 + 255) / 256) < 148ll * 16 ? ((total16 + 255) / 256) : 148ll * 16);
+    const int grid = static_cast<int>(((total16 + 255) / 256) < 132ll * 16 ? ((total16 + 255) / 256) : 132ll * 16);
     pack_gate_up_kernel<<<grid, 256, 0, stream>>>(gate, up, packed, F, K, total16);
     AF3_CHECK_LAUNCH();
     return 0;
@@ -434,7 +434,7 @@ int rope_kv_append(cudaStream_t stream, bf16* qkv, bf16* k_cache, bf16* v_cache,
     if (tok_chunks <= 0) return 0;
     const bool head_par = tok_chunks < 8192;  // decode steps / short prompts
     const long long total = tok_chunks * (head_par ? (H + 2 * Hkv) : 1);
-    const int grid = static_cast<int>(((total + 255) / 256) < 148ll * 32 ? ((total + 255) / 256) : 148ll * 32);
+    const int grid = static_cast<int>(((total + 255) / 256) < 132ll * 32 ? ((total + 255) / 256) : 132ll * 32);
     if (head_par)
         AF3_CHECK_CUDA(launch_kernel(rope_kv_append_kernel<true>, dim3(grid), dim3(256), 0, stream, qkv, k_cache, v_cache, B, T, H,
                                      Hkv, D, Tmax, pos0, pos0_dev, kv_start, inv_freq));
@@ -485,7 +485,7 @@ int rotary_time(cudaStream_t stream, bf16* x, const float* ts, const float* inv_
     AF3_REQUIRE(4 * n_freq <= dim && n_freq > 0, "rotary_time: rotary width exceeds the feature dim");
     const long long total = static_cast<long long>(W) * T * 2 * n_freq;
     if (total <= 0) return 0;
-    const int grid = static_cast<int>(((total + 255) / 256) < 148ll * 16 ? ((total + 255) / 256) : 148ll * 16);
+    const int grid = static_cast<int>(((total + 255) / 256) < 132ll * 16 ? ((total + 255) / 256) : 132ll * 16);
     rotary_time_kernel<<<grid, 256, 0, stream>>>(x, ts, inv_freq, W, T, dim, n_freq, window_duration, max_len);
     AF3_CHECK_LAUNCH();
     return 0;

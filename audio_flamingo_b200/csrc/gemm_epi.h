@@ -1,4 +1,4 @@
-// Epilogue flags and side-argument structs shared by the GEMM translation units (gemm_tcgen05.cu) and
+// Epilogue flags and side-argument structs shared by the GEMM translation units (gemm_wgmma.cu) and
 // the C ABI (af3_abi.cu); the flag values are the AF3_EPI_* constants of include/af3b200.h.
 #pragma once
 #include "common.h"
@@ -17,7 +17,7 @@ struct RopeEpilogue {
     int H, Hkv, Tmax;
 };
 
-// RMSNorm fusion across few-token GEMMs (see GemmArgs in gemm_tcgen05.cu): consumer side (norm_w ...) and / or producer side (sumsq_out ...)
+// RMSNorm fusion across few-token GEMMs (see GemmArgs in gemm_wgmma.cu): consumer side (norm_w ...) and / or producer side (sumsq_out ...)
 struct NormFusion {
     const bf16* norm_w;
     const float* norm_part;

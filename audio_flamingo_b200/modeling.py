@@ -1,4 +1,4 @@
-"""B200-native Audio Flamingo 3 forward path behind the reference's PyTorch module surface.
+"""H100-native Audio Flamingo 3 forward path behind the reference's PyTorch module surface.
 
 Mirrors (class roles, forward/generate/get_audio_features signatures, state_dict key names) the executable
 reference of this path, transformers 5.5.0 ([O], SURVEY.md 2.3):
@@ -8,7 +8,7 @@ reference of this path, transformers 5.5.0 ([O], SURVEY.md 2.3):
     AudioFlamingo3ForConditionalGeneration    [O] AF3M:410-592 (+ greedy loop GEN:2658-2812)
 The nn.Module tree below only *holds* parameters under the reference's names (so `load_state_dict` of a reference
 checkpoint works unchanged); no nn.Module.forward of torch is ever executed.  All arithmetic runs in the hand-written
-sm_100a kernels of libaf3b200.so through audio_flamingo_b200.ops; this file is launch orchestration, buffer
+sm_90a kernels of libaf3b200.so through audio_flamingo_b200.ops; this file is launch orchestration, buffer
 management (torch caching allocator, current CUDA stream) and CUDA-graph capture of the decode step.
 Compute dtype: bf16 parameters/activations, fp32 accumulation/statistics, fp32 logits -- same as running the
 reference with model.to(torch.bfloat16).
@@ -97,7 +97,7 @@ class AudioFlamingo3Encoder(nn.Module):
         self.d_model, self.n_heads, self.ffn = d, config.num_attention_heads, config.intermediate_size
         self.head_dim = d // self.n_heads
         if self.head_dim not in (64, 128):
-            raise AF3Error("encoder head_dim must be 64 or 128 for the tcgen05 attention kernel")
+            raise AF3Error("encoder head_dim must be 64 or 128 for the wgmma attention kernel")
         self.num_mel_bins = config.num_mel_bins
         self.max_source_positions = config.max_source_positions
         if _cfg_get(config, "activation_function", "gelu") != "gelu" or _cfg_get(config, "scale_embedding", False):
@@ -286,8 +286,8 @@ class AF3KVCache:
 
 
 class Qwen2ForCausalLM(nn.Module):
-    """Decoder ([O] Q2M:332-487) on sm_100a kernels: RMSNorm, fused QKV GEMM (+bias), RoPE + in-place KV append,
-    tcgen05 causal GQA attention (prefill) / split-KV decode attention, o GEMM (+residual), fused SwiGLU GEMM,
+    """Decoder ([O] Q2M:332-487) on sm_90a kernels: RMSNorm, fused QKV GEMM (+bias), RoPE + in-place KV append,
+    wgmma causal GQA attention (prefill) / split-KV decode attention, o GEMM (+residual), fused SwiGLU GEMM,
     down GEMM (+residual), final norm, LM head to fp32 logits."""
 
     def __init__(self, tc):
@@ -355,9 +355,9 @@ class Qwen2ForCausalLM(nn.Module):
         fused_qkv = decode and B <= 64  # few-token ("swapped") GEMM with RoPE + KV append in its epilogue
         # Decode step with RMSNorm fused ACROSS the GEMMs (include/af3b200.h af3_gemm_fusion): the residual GEMMs (o, down) emit the
         # per-row-tile sums of squares of the rows they store, the next q/k/v / gate-up GEMM normalises its activation tiles in shared
-        # memory; 55 of the 57 norm launches of a step disappear.  OPT-IN (AF3_FUSE_NORM=1): parity-clean, but measured 3-7 % SLOWER
-        # than the chain with stand-alone norm kernels in four A/B runs (profiles/r02g..i_decode_timeline_*): the few-token streams
-        # are latency-bound on ring depth, and a stage that waits for its activation tile to be rewritten is a stage not in flight.
+        # memory; 55 of the 57 norm launches of a step disappear.  OPT-IN (AF3_FUSE_NORM=1): parity-clean, but not shown to be faster
+        # than the chain with stand-alone norm kernels: the few-token streams are latency-bound on ring depth, and a stage that waits
+        # for its activation tile to be rewritten is a stage not in flight.
         fuse_norm = fused_qkv and self.hid % 64 == 0 and self.hid <= 4096 and os.environ.get("AF3_FUSE_NORM", "0") == "1"
         n_parts = -(-self.hid // 128)
         if fused_qkv:
@@ -709,7 +709,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                 continue
             if k in self._ACCEPTED_DEFAULTS and (v == self._ACCEPTED_DEFAULTS[k] or v is None):
                 continue
-            raise AF3Error(f"generate(): option {k}={v!r} is not implemented on the B200 greedy path "
+            raise AF3Error(f"generate(): option {k}={v!r} is not implemented on the greedy GPU path "
                            "(greedy decoding, one sequence per prompt, no logits processors)")
         if do_sample is None:
             do_sample = bool(self._generation_default("do_sample"))

@@ -1,4 +1,4 @@
-"""Flamingo-style gated cross-attention + gated dense block on the B200 kernels (SURVEY.md 8-f.4, BASELINE config 4).
+"""Flamingo-style gated cross-attention + gated dense block on the sm_90a kernels (SURVEY.md 8-f.4, BASELINE config 4).
 
 Audio Flamingo 2 conditions a frozen decoder on sliding-window audio features through such blocks placed before the decoder
 layers (arXiv 2503.03983, after Flamingo, arXiv 2204.14198).  The `audio_flamingo_2` branch is NOT in the mounted reference and
@@ -58,7 +58,7 @@ class GatedCrossAttentionLayer(nn.Module):
         self.hidden, self.heads, self.inter, self.media_dim, self.eps = hidden_size, num_attention_heads, intermediate_size, media_dim, rms_norm_eps
         self.head_dim = hidden_size // num_attention_heads
         if self.head_dim not in (64, 128):
-            raise AF3Error("head_dim must be 64 or 128 for the tcgen05 attention kernel")
+            raise AF3Error("head_dim must be 64 or 128 for the wgmma attention kernel")
         if alpha_type not in ("vector", "float"):
             raise AF3Error("alpha_type must be 'vector' or 'float'")
         self.cross_attn = _XAttn(hidden_size, num_attention_heads, media_dim)

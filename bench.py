@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- AF3-7B audio->text hot path on B200 (driver contract; see DESIGN.md "Measurement").
+"""bench.py -- AF3-7B audio->text hot path on H100 (see DESIGN.md "Measurement").
 
 Workload (BASELINE.json configs[1]): AF3-7B, batch 32 x 30 s clips per GPU, greedy 128-token decode.
 One "step" = one pass of the whole path over one batch of synthetic audio:
@@ -110,7 +110,7 @@ def measured_peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "MEASURED_PEAKS.json (of measured)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "B200_PROFILING.md fallback (of fallback)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet (700 W), not measured"}
 
 
 def af3_config():
@@ -164,7 +164,7 @@ def _cuda_ms(fn, warm=1, iters=2):
 
 def gpu_reference(model, cfg, dev, feats, fmask, ids, our_stage_ms, our_ms_step):
     """The number the kernels have to beat (SURVEY 8-d, BASELINE.md 3): the reference's own implementation of the path -- unmodified HF
-    transformers classes, eager bf16, attn_implementation sdpa -- on the SAME B200, SAME weights (parameters are shared with our model
+    transformers classes, eager bf16, attn_implementation sdpa -- on the SAME GPU, SAME weights (parameters are shared with our model
     through load_state_dict(assign=True): no second copy), same batch: per stage and for the whole generate() call."""
     import transformers
     from transformers import AudioFlamingo3ForConditionalGeneration as HFModel
@@ -279,7 +279,7 @@ def run_ours(args):
         out = gather_tokens(out, assume_equal_length=True)   # the path's only collective (NCCL all-gather of int64 ids; no EOS here)
         if from_host:
             tokens_host.copy_(out, non_blocking=True)  # D2H read of the step's result
-        return out
+        return out, feats["input_features"]
 
     def barrier():
         if world > 1:
@@ -289,6 +289,7 @@ def run_ours(args):
         torch.cuda.synchronize()
 
     host_t = []  # per timed step: [(stage name, host perf_counter when that stage boundary was ENQUEUED)]
+    last = {}    # what the last timed step returned (--dump-outputs)
 
     def timed(n_steps, from_host, collect_stages=False):
         barrier()
@@ -303,7 +304,7 @@ def run_ours(args):
                 ev.record()
                 model.stage_events.append(("step_start", ev))
                 model.stage_host_t = []
-            step(from_host)
+            last["ids"], last["feats"] = step(from_host)
             if collect_stages:
                 stages.append(model.stage_events)
                 host_t.append(model.stage_host_t)
@@ -335,6 +336,8 @@ def run_ours(args):
         sampler.start()
     thr0 = cpu_throttle_snapshot()
     ms_dev, launches, stages = timed(args.steps, from_host=False, collect_stages=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["ids"], last["feats"])
     thr1 = cpu_throttle_snapshot()
     host_cpu = {"cpus_allowed": len(os.sched_getaffinity(0)), "loadavg": os.getloadavg()[0],
                 "throttled_during_timed": None if (thr0 is None or thr1 is None) else
@@ -522,14 +525,14 @@ def run_ours(args):
             flops = 2.0 * a * n_feat_w * c
             # few-token GEMM: the weight matrix is the traffic (read once); activations / outputs are < 1 % of it
             bytes_alg = 2.0 * n_feat_w * c if a <= 64 else 2.0 * (a * c + n_feat_w * c + a * b)
-            row.update({"kernel": "gemm_tcgen05" + ("(swap)" if a <= 64 else ""), "n_tok": a, "n_feat": b, "K": c, "flags": flags,
+            row.update({"kernel": "gemm_wgmma" + ("(swap)" if a <= 64 else ""), "n_tok": a, "n_feat": b, "K": c, "flags": flags,
                         "tflops": flops * n / (tot * 1e-3) / 1e12, "gbs": bytes_alg * n / (tot * 1e-3) / 1e9,
                         "flops_per_launch": flops, "bytes_per_launch": bytes_alg, "bound": "hbm" if a <= 64 else "tensor"})
         elif kind == "attention":
             D = flags // 2
             causal = flags & 1
             flops = 4.0 * a * b * c * D * (0.5 if causal else 1.0)
-            row.update({"kernel": "attention_tcgen05", "bh": a, "Tq": b, "Tk": c, "D": D, "causal": causal,
+            row.update({"kernel": "attention_wgmma", "bh": a, "Tq": b, "Tk": c, "D": D, "causal": causal,
                         "tflops": flops * n / (tot * 1e-3) / 1e12, "flops_per_launch": flops, "bound": "tensor"})
         elif kind == "decode_attention":
             # a = sequences, b = query heads, c = cache capacity; K and V of the live context (prompt + 1 here) once: 4 KV heads x 128 x 2 B x 2
@@ -584,7 +587,7 @@ def run_ours(args):
     rated = [r for r in table if "bound" in r]
     top = rated[0] if rated else None
     roofline = roofline_of(top, "gemm_decode_traffic_bytes" if (top and top["kernel"].endswith("(swap)")) else "gemm_prefill_traffic_bytes")
-    top_prefill = next((r for r in rated if r["kernel"] == "gemm_tcgen05"), None)
+    top_prefill = next((r for r in rated if r["kernel"] == "gemm_wgmma"), None)
     roofline_prefill_gemm = roofline_of(top_prefill, "gemm_prefill_traffic_bytes")
     # decode-step HBM roofline (whole step): weights once + KV of the live context
     dec_bytes = 2.0 * (6525618176 + 544997376) + 57344.0 * (S_prompt + NEW_TOKENS // 2) * B
@@ -819,12 +822,27 @@ def run_reference(args):
     print(json.dumps(line))
 
 
+def dump_outputs(out_dir, ids, feats):
+    """What the last timed step returned to its caller: the generated ids (all of them, as float64, exact) and a fixed seeded
+    sample of 2^20 log-mel features (float32) with their flat indices -- about 13 MB in all, comparable output for output between
+    two builds."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "generated_ids.npy", ids.cpu().numpy().astype(np.float64))
+    f = feats.float().reshape(-1).cpu().numpy()
+    idx = np.sort(np.random.RandomState(0).choice(f.size, size=min(f.size, 1 << 20), replace=False))
+    np.save(d / "input_features_sample.npy", f[idx].astype(np.float32))
+    np.save(d / "input_features_sample_index.npy", idx.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (generated ids, a log-mel sample) as DIR/<name>.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true", help="skip timing HF transformers (eager bf16) on the same GPU")
     ap.add_argument("--no-extras", action="store_true", help="skip the BASELINE config 3 / config 5 / 256-window log-mel measurements")

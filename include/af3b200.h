@@ -1,4 +1,4 @@
-/* libaf3b200.so -- C ABI of the B200-native Audio Flamingo 3 audio->text hot path.
+/* libaf3b200.so -- C ABI of the H100-native (sm_90a) Audio Flamingo 3 audio->text hot path.
  *
  * Boundary (SURVEY.md 8-b): the reference path sits behind PyTorch nn.Module call conventions, not an FFI
  * registry, so there is no pre-existing binding to copy.  Each entry point below names the reference interface
@@ -54,7 +54,7 @@ int af3_trace_seq(void);
 #define AF3_EPI_F32OUT 16
 #define AF3_EPI_SWIGLU_CONCAT 64 /* with AF3_EPI_SWIGLU: w is [gate (n_feat rows); up (n_feat rows)], n_feat % 128 == 0 */
 
-/* out[tok, feat] = epi( x[tok,:] . w[feat,:] ), tcgen05 tensor cores.  Replaces F.linear at
+/* out[tok, feat] = epi( x[tok,:] . w[feat,:] ), wgmma tensor cores.  Replaces F.linear at
  * [O] AF3M:111-114,141,153-154,204-205,398-402; Q2M:41-48,199-202,474-475 and F.conv1d (as im2col GEMM) at
  * AF3M:343-344.  With AF3_EPI_SWIGLU, w holds gate/up rows interleaved in blocks of 128 (see af3_pack_gate_up) -- or, with
  * AF3_EPI_SWIGLU_CONCAT, simply concatenated [gate; up] (so the two nn.Linear weights can be views of one matrix) --
@@ -99,7 +99,7 @@ int af3_avgpool_layernorm(void* stream, const void* x, void* y, const void* gamm
 int af3_rmsnorm(void* stream, const void* x, void* y, const void* weight, int rows, int dim, float eps,
                 const int* row_idx);
 
-/* Bidirectional / causal softmax attention on tcgen05 (replaces SDPA:40-104 as called from AF3M:170-181 and
+/* Bidirectional / causal softmax attention on wgmma (replaces SDPA:40-104 as called from AF3M:170-181 and
  * Q2M:227-238).  q rows come from a packed projection buffer: q[b, t, h*D + d] at q + (b*Tq + t)*ldq.
  * k, v: element (b, hk, t, d) at k + ((b*Hkv + hk)*Tk_pitch + t)*ldk + d  when kv_layout = 1 (cache layout), or
  * (b, t, hk*D + d) at k + (b*Tk + t)*ldk when kv_layout = 0 (packed projection buffer).
@@ -139,7 +139,7 @@ int af3_rope_table(void* stream, float* rope_cs, int B, int D, const int* pos_de
                    const float* inv_freq);
 
 /* Qwen2RMSNorm ([O] Q2M:258-263) fused ACROSS two few-token (n_tok <= 64) GEMMs of the decode step, so that the norm kernel and
- * its two dependency hops leave the step's kernel chain (profiles/r02b_decode_timeline.md: 57 norm launches x 2.9 us per step):
+ * its two dependency hops leave the step's kernel chain:
  *   producer side (a GEMM with the bf16 token-major epilogue, typically the residual o / down projection): sumsq_out
  *     [n_tok][sumsq_ld] receives, per token, one sum of squares per 128-feature row tile (entry [tok][tile]) of the bf16
  *     values the GEMM stored;
@@ -147,8 +147,7 @@ int af3_rope_table(void* stream, float* rope_cs, int B, int D, const int* pos_de
  *     producer's partials (norm_sumsq [n_tok][norm_ld], the first norm_parts <= 32 entries of a row are summed, norm_ld >= 32 and a
  *     multiple of 4, rows 16-byte aligned) the kernel computes rstd = rsqrt(sum / K + eps) per token and feeds the tensor cores
  *     norm_weight[k] * bf16(x[k] * rstd)  -- the reference's two roundings -- instead of x.
- * Either side may be left out (NULL pointers).  K % 64 == 0; the consumer must fit one work item per SM (true for the decode
- * shapes; checked).  Deterministic (fixed summation order). */
+ * Either side may be left out (NULL pointers).  K % 64 == 0.  Deterministic (fixed summation order). */
 typedef struct af3_gemm_fusion {
     const void* norm_weight; /* bf16 [K] or NULL */
     const float* norm_sumsq; /* [n_tok][norm_ld], norm_parts used per row */

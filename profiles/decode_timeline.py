@@ -1,14 +1,13 @@
 #!/usr/bin/env python
 """In-graph timeline of one decode step (programmatic dependent launch ON, nothing serialised).
 
-ncu replays kernels one at a time, so it cannot show where the decode step's slack sits (VERDICT r01: 3.67 ms per step
-against a 2.39 ms HBM bound).  This tool opens the library's trace (include/af3b200.h: af3_trace_begin), runs
+Nsight Compute replays kernels one at a time, so it cannot show where the decode step's slack sits.  This tool opens the library's trace (include/af3b200.h: af3_trace_begin), runs
 generate() at the bench's shape (AF3-7B decoder, 32 sequences, 780-token prompts) so that the decode step is captured
 in a CUDA graph WITH the trace slots baked in, replays it, and reads back per-CTA %globaltimer stamps of the LAST replay:
     mark 0 kernel entry, 1 after griddepcontrol.wait, 2 main loop done (GEMM: last accumulator ready), 3 exit.
 Output: JSON (one record per launch + per-kind aggregates) and a markdown summary.
 
-    python profiles/decode_timeline.py --out profiles/r02_decode_timeline --tag stages8
+    python profiles/decode_timeline.py --out /tmp/decode_timeline --tag base
 Environment knobs under test are simply inherited (AF3_PDL, AF3_FUSE_NORM, AF3_L2_PREFETCH*, AF3_KSPLIT, ...).
 """
 from __future__ import annotations
@@ -17,6 +16,7 @@ import argparse
 import json
 import os
 import sys
+import tempfile
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -28,7 +28,7 @@ import torch  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", default=str(ROOT / "profiles" / "r02_decode_timeline"))
+    ap.add_argument("--out", default=str(Path(tempfile.gettempdir()) / "decode_timeline"))
     ap.add_argument("--tag", default="default")
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--prompt", type=int, default=780)

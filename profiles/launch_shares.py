@@ -1,6 +1,6 @@
 """ncu launch list (gpu__time_duration.sum per launch, one profiled bench step with a few EAGER decode steps) -> shares of the step
 with the decode-step kernels weighted to the 127 steps of the real workload (VERDICT r01: the raw list under-weights decode ~40 x).
-    python profiles/launch_shares.py gpurun_out/launches.csv profiles/r02_launch_shares.md"""
+    python profiles/launch_shares.py launches.csv launch_shares.md"""
 import collections
 import csv
 import re

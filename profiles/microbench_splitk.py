@@ -1,8 +1,7 @@
 """Few-token (decode) GEMM: time per launch and its split into weight streaming vs reduction/epilogue tail, as a function of the
-number of K splits.  The decode-step timeline (profiles/r02_decode_timeline_*.md) showed the split-K tails (last accumulator ready
--> last CTA exit: 6-7 us for q/k/v, o and down) to be the largest loss of the step; this sweep measures (a) how the tail scales with
-the split count and (b) whether fewer CTAs (72 at 2 splits) still pull the weights at HBM speed.
-    python profiles/microbench_splitk.py > gpurun_out/splitk.json
+number of K splits (the split-K tail: last accumulator ready -> last CTA exit); this sweep measures (a) how the tail scales with
+the split count and (b) whether fewer CTAs still pull the weights at HBM speed.
+    python profiles/microbench_splitk.py > splitk.json
 us per launch: CUDA events around a graph of 48 back-to-back launches (no PDL), weights rotated over 12 copies so every launch
 streams from HBM.  stream / tail: library trace (%globaltimer) of 12 eager launches, medians."""
 import json
@@ -79,7 +78,7 @@ def run_shape(name, N, K, mode, copies=12, iters=48):
         del g
     os.environ.pop("AF3_KSPLIT", None)
     os.environ.pop("AF3_CLUSTER_REDUCE", None)
-    return {"shape": name, "n_feat": N, "K": K, "epilogue": mode, "weight_bytes": N * K * 2, "ideal_us_at_6573_gbs": round(N * K * 2 / 6573e3, 2),
+    return {"shape": name, "n_feat": N, "K": K, "epilogue": mode, "weight_bytes": N * K * 2, "ideal_us_at_3350_gbs": round(N * K * 2 / 3350e3, 2),   # H100 SXM data-sheet HBM3 bandwidth
             "sweep": rows}
 
 

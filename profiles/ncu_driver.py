@@ -1,4 +1,4 @@
-"""Driver for the ncu passes (profiling recipe, /opt/skills/guides/B200_PROFILING.md): builds the bench workload,
+"""Runner for Nsight Compute passes: builds the bench workload,
 runs warm-up steps unprofiled, then ONE step between cudaProfilerStart/Stop.
   launch list : ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none -c 1600 --csv --log-file X python profiles/ncu_driver.py
   top kernel  : ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:gemm_kernel -c 3 -o X python profiles/ncu_driver.py

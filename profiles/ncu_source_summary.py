@@ -54,7 +54,7 @@ def main():
         elif "TRYWAIT" in s_ or (s_.startswith("@") and "BRA" in s_ and near_wait) or "YIELD" in s_ or "NANOSLEEP" in s_:
             grp["mbarrier wait loops"] += s
         else:
-            grp["everything else (compute, TMEM, stores)"] += s
+            grp["everything else (compute, stores)"] += s
             for k, v in st.items():
                 other_st[k] += v
     lines = [f"# ncu source-level summary: `{kname[:140]}`", "", f"report: `{rep}` (ncu --set full --clock-control none --import-source on, one launch).  {note}", ""]
@@ -64,7 +64,8 @@ def main():
             lines.append(f"| {k} | {metric[k][0]} {metric[k][1]} |")
     cyc = float(metric.get("sm__cycles_elapsed.max", ("0", ""))[0] or 0)
     if cyc:
-        lines.append(f"| warp instructions executed / (cycles x 148 SMs x 4 schedulers) | {n_inst} / {cyc * 592:.0f} = {n_inst / (cyc * 592):.3f} IPC per scheduler |")
+        sched = 132 * 4   # H100 SXM: 132 SMs x 4 schedulers
+        lines.append(f"| warp instructions executed / (cycles x 132 SMs x 4 schedulers) | {n_inst} / {cyc * sched:.0f} = {n_inst / (cyc * sched):.3f} IPC per scheduler |")
     lines += ["", f"Warp-state samples: {tot}", "", "| where | share |", "|---|---|"]
     for k, v in grp.most_common():
         lines.append(f"| {k} | {100 * v / tot:.1f} % |")

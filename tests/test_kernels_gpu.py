@@ -78,7 +78,15 @@ def test_gemm_splitk_deterministic_and_epilogue(ops):
     # one bf16 ulp of the (larger) linear output may survive the residual add even where lin + res cancels
     err = (outs[0].float() - ref.float()).abs()
     tol = 4e-3 + BF16_RTOL * (lin.abs() + res.float().abs())
-    assert (err <= tol).all(), f"max err {err.max().item()}"
+    # Where the fp32 accumulator sits on a bf16 rounding tie of lin, another summation order rounds lin one ulp the other way and
+    # the second rounding (after the residual add) can turn that into two ulps of the output.  Such elements must be rare and
+    # exactly the reference's two roundings applied to this kernel's own linear output, itself within one ulp of lin.
+    off = err > tol
+    assert int(off.sum()) <= 8, f"{int(off.sum())} elements out of tolerance, max err {err.max().item()}"
+    if off.any():
+        lin_k = ops.linear(x, w).float()
+        assert torch.equal(outs[0][off], (lin_k[off] + res.float()[off]).to(bf16)), "fused residual epilogue != its unfused chain"
+        assert ((lin_k - lin).abs()[off] <= BF16_RTOL * lin.abs()[off]).all(), f"max err {err.max().item()}"
 
 
 @pytest.mark.parametrize("M", [16, 640])
@@ -186,7 +194,7 @@ def test_im2col(ops):
 
 
 def test_conv_stem_as_gemm(ops):
-    """conv1d(k3,p1)+GELU and conv1d(k3,s2,p1)+GELU through im2col + tcgen05 GEMM vs F.conv1d."""
+    """conv1d(k3,p1)+GELU and conv1d(k3,s2,p1)+GELU through im2col + wgmma GEMM vs F.conv1d."""
     n_win, C, T, Dm = 2, 128, 200, 256
     x = _rand((n_win, C, T), 1.0, 28, torch.float32)
     w1, b1 = _rand((Dm, C, 3), 0.05, 29), _rand((Dm,), 0.1, 30)
@@ -210,18 +218,17 @@ def _sdpa_ref(q, k, v, scale, mask):
     return p @ v
 
 
-@pytest.fixture(params=["v2", "v2_tpr2", "v1"])
+@pytest.fixture(params=["v2", "v1"])
 def attn_impl(request, monkeypatch):
-    """All variants of the prefill / encoder attention kernel go through the same parity cases: v2 (two Q tiles per CTA, P in
-    tensor memory; one softmax thread per row = the default, two per row = AF3_ATTN_TPR=2) and the round-1 kernel
-    (AF3_ATTN_V1=1, kept as cross-check)."""
+    """Both row tilings of the prefill / encoder attention kernel go through the same parity cases: v2 (two consumer warpgroups,
+    128 query rows per CTA = the default) and v1 (one warpgroup, 64 rows per CTA: AF3_ATTN_V1=1, kept as cross-check)."""
     monkeypatch.setenv("AF3_ATTN_V1", "1" if request.param == "v1" else "0")
-    monkeypatch.setenv("AF3_ATTN_TPR", "2" if request.param == "v2_tpr2" else "1")
     return request.param
 
 
 @pytest.mark.parametrize("D,H,T,lens", [(64, 4, 200, None), (64, 20, 1500, None), (64, 3, 333, [333, 100, 7]), (128, 2, 256, None),
-                                        (64, 2, 1500, [1500, 385, 12]), (128, 3, 700, [700, 129, 256])])
+                                        (64, 2, 1500, [1500, 385, 12]), (128, 3, 700, [700, 129, 256]), (64, 2, 65, None),
+                                        (128, 2, 300, [300, 1, 190]), (64, 5, 2000, [2000, 1999, 640])])
 def test_attention_bidirectional(ops, attn_impl, D, H, T, lens):
     B = 3 if lens else 2
     qkv = _rand((B * T, 3 * H * D), 1.0, 40)
@@ -239,7 +246,8 @@ def test_attention_bidirectional(ops, attn_impl, D, H, T, lens):
     _close(out, ref, 2e-2, 2e-2, f"attention D={D} T={T}")
 
 
-@pytest.mark.parametrize("T,starts", [(256, None), (300, [0, 37, 250]), (130, [5, 129]), (780, [0, 3, 530]), (1000, None)])
+@pytest.mark.parametrize("T,starts", [(256, None), (300, [0, 37, 250]), (130, [5, 129]), (780, [0, 3, 530]), (1000, None), (64, None),
+                                      (129, [0, 128]), (513, [0, 400, 512])])
 def test_attention_causal_gqa_cache(ops, attn_impl, T, starts):
     H, Hkv, D, Tmax = 8, 2, 128, 1024
     B = len(starts) if starts else 2

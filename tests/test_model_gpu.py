@@ -1,4 +1,4 @@
-"""End-to-end parity on the GPU: the B200 path vs the unmodified HF reference (same seeded synthetic weights) run
+"""End-to-end parity on the GPU: the H100 path vs the unmodified HF reference (same seeded synthetic weights) run
 (a) in bf16 on the same GPU -- the reference's own PyTorch path in the same dtype -- and (b) in fp32 (oracle
 restatement / HF fp32).  Tolerances: logits are bf16-rounded values with |logit| up to ~10 at sharpen=8; bf16 GEMM
 chains of 2..32 layers give ~1e-2 relative noise, so we require max|diff| <= 6% of the logit std and compare our

@@ -1,4 +1,4 @@
-"""SURVEY 8-f.4 (AF2's LM-side conditioning): the gated cross-attention + gated dense block on the B200 kernels vs the executable
+"""SURVEY 8-f.4 (AF2's LM-side conditioning): the gated cross-attention + gated dense block on the H100 kernels vs the executable
 analogue of that operator, transformers' IdeficsGatedCrossAttentionLayer ([O] idefics/modeling_idefics.py:684-806), run in bf16 on
 the same GPU and in fp32 on the CPU (same seeded weights).  AF2 itself stays unpinned: see oracle/af2_oracle.py.
 Tolerance: bf16 outputs of O(1..5); ours must not be further from fp32 than 1.5x the analogue's own bf16 run (floor 2 % of max |ref|)."""
