@@ -38,8 +38,7 @@ SIGNATURES = {
     "af3_rotary_time_emb": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _f, _f]),
     "af3_rope_table": (_i, [_p, _p, _i, _i, _p, _p, _p]),
     "af3_gated_residual": (_i, [_p, _p, _p, _p, _i, _p, _p, _i, _i]),
-    "af3_gemm_qkv_rope": (_i, [_p, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz, _p]),
-    "af3_gemm_bf16_fused": (_i, [_p, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _i, _i, _p, _sz, _p]),
+    "af3_gemm_qkv_rope": (_i, [_p, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz]),
     "af3_decode_attention": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _f]),
     "af3_decode_attention_scratch_bytes": (_sz, [_i, _i, _i, _i]),
     "af3_embed_scatter": (_i, [_p, _p, _i, _p, _i, _i64, _p, _i, _i, _p, _p, _p, _p]),
@@ -47,12 +46,6 @@ SIGNATURES = {
     "af3_argmax": (_i, [_p, _p, _i, _i, _p, _p]),
     "af3_token_step": (_i, [_p, _p, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
 }
-
-class GemmFusion(C.Structure):
-    """af3_gemm_fusion (include/af3b200.h): RMSNorm fused across two few-token GEMMs."""
-
-    _fields_ = [("norm_weight", C.c_void_p), ("norm_sumsq", C.c_void_p), ("norm_parts", C.c_int), ("norm_ld", C.c_int),
-                ("norm_eps", C.c_float), ("sumsq_out", C.c_void_p), ("sumsq_ld", C.c_int)]
 
 
 _lib = None

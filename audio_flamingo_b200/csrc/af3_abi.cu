@@ -47,7 +47,7 @@ using af3::bf16;
 extern "C" {
 
 const char* af3_last_error(void) { return af3::last_error_cstr(); }
-int af3_abi_version(void) { return 3; }
+int af3_abi_version(void) { return 4; }
 void af3_set_pdl(int enable) { af3::set_pdl(enable != 0); }
 size_t af3_trace_slot_bytes(void) { return sizeof(unsigned long long) * af3::TRACE_CTAS * af3::TRACE_MARKS; }
 int af3_trace_begin(void* buf, size_t bytes) { return af3::trace_begin(buf, bytes); }
@@ -57,7 +57,7 @@ int af3_trace_seq(void) { return af3::trace_seq(); }
 int af3_gemm_bf16(void* stream, const void* x, int ldx, const void* w, int ldw, void* out, int ldo, int n_tok, int n_feat,
                   int K, int flags, const void* bias, const void* resid, int ld_res, int res_period) {
     return af3::gemm_bf16(S(stream), B16(x), ldx, B16(w), ldw, out, ldo, n_tok, n_feat, K, flags, B16(bias), B16(resid),
-                          ld_res, res_period, nullptr, 0, nullptr, nullptr);
+                          ld_res, res_period, nullptr, 0, nullptr);
 }
 
 size_t af3_gemm_workspace_bytes(void) { return af3::gemm_workspace_bytes(); }
@@ -66,29 +66,7 @@ int af3_gemm_bf16_ws(void* stream, const void* x, int ldx, const void* w, int ld
                      int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res, int res_period,
                      void* workspace, size_t workspace_bytes) {
     return af3::gemm_bf16(S(stream), B16(x), ldx, B16(w), ldw, out, ldo, n_tok, n_feat, K, flags, B16(bias), B16(resid),
-                          ld_res, res_period, workspace, workspace_bytes, nullptr, nullptr);
-}
-
-static af3::NormFusion to_nf(const af3_gemm_fusion* f) {
-    af3::NormFusion n{};
-    if (f) {
-        n.norm_w = B16(f->norm_weight);
-        n.norm_part = f->norm_sumsq;
-        n.norm_parts = f->norm_parts;
-        n.norm_ld = f->norm_ld;
-        n.norm_eps = f->norm_eps;
-        n.sumsq_out = f->sumsq_out;
-        n.sumsq_ld = f->sumsq_ld;
-    }
-    return n;
-}
-
-int af3_gemm_bf16_fused(void* stream, const void* x, int ldx, const void* w, int ldw, void* out, int ldo, int n_tok,
-                        int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res, int res_period,
-                        void* workspace, size_t workspace_bytes, const af3_gemm_fusion* fusion) {
-    const af3::NormFusion n = to_nf(fusion);
-    return af3::gemm_bf16(S(stream), B16(x), ldx, B16(w), ldw, out, ldo, n_tok, n_feat, K, flags, B16(bias), B16(resid),
-                          ld_res, res_period, workspace, workspace_bytes, nullptr, fusion ? &n : nullptr);
+                          ld_res, res_period, workspace, workspace_bytes, nullptr);
 }
 
 int af3_rotary_time_emb(void* stream, void* x, const float* timestamps, const float* inv_freq, int W, int T, int dim, int n_freq,
@@ -107,13 +85,11 @@ int af3_rope_table(void* stream, float* cs, int B, int D, const int* pos_dev, co
 
 int af3_gemm_qkv_rope(void* stream, const void* x, int ldx, const void* w, int ldw, const void* bias, void* q_out, int ldo,
                       int n_tok, int K, int H, int Hkv, int D, const float* rope_cs, void* k_cache, void* v_cache, int Tmax,
-                      const int* pos_dev, void* workspace, size_t workspace_bytes, const af3_gemm_fusion* fusion) {
+                      const int* pos_dev, void* workspace, size_t workspace_bytes) {
     if (D != 128) return af3::fail("af3_gemm_qkv_rope: head_dim must be 128");
-    if (fusion && fusion->sumsq_out) return af3::fail("af3_gemm_qkv_rope: only the consumer side of the RMSNorm fusion applies here");
     af3::RopeEpilogue r{rope_cs, B16M(k_cache), B16M(v_cache), pos_dev, H, Hkv, Tmax};
-    const af3::NormFusion n = to_nf(fusion);
     return af3::gemm_bf16(S(stream), B16(x), ldx, B16(w), ldw, q_out, ldo, n_tok, (H + 2 * Hkv) * D, K,
-                          AF3_EPI_BIAS | 32, B16(bias), nullptr, 0, 0, workspace, workspace_bytes, &r, fusion ? &n : nullptr);
+                          AF3_EPI_BIAS | 32, B16(bias), nullptr, 0, 0, workspace, workspace_bytes, &r);
 }
 
 int af3_pack_gate_up(void* stream, const void* gate, const void* up, void* packed, int F, int K) {

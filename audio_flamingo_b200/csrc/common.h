@@ -76,50 +76,6 @@ inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, 
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
-// Same, as thread-block clusters of `cluster_x` consecutive CTAs (grid.x must be a multiple of it): the CTAs of a cluster are
-// co-scheduled on one GPC and can address each other's shared memory (DSMEM).
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_kernel_cluster(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                                         int cluster_x, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster_x;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
-
-// How many clusters of `cluster_x` CTAs of this kernel can be resident at once on the current device (0 on error).
-template <typename... KArgs>
-inline int max_active_clusters(void (*kern)(KArgs...), dim3 block, size_t smem, int cluster_x) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(cluster_x * 64);
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster_x;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, reinterpret_cast<const void*>(kern), &cfg) != cudaSuccess) {
-        cudaGetLastError();
-        return 0;
-    }
-    return n;
-}
-
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 // In-graph timeline of the decode-step kernel chain (af3_trace_begin / af3_trace_end, profiles/decode_timeline.py).

@@ -114,7 +114,7 @@ __global__ void __launch_bounds__(DA_THREADS, 1)
 decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                    const __grid_constant__ CUtensorMap map_v, float* __restrict__ part, bf16* __restrict__ out,
                    int* __restrict__ counters, int H, int Hkv, int nz, const int* __restrict__ ctx_len_p,
-                   const int* __restrict__ kv_start, float scale_log2, unsigned long long* trace, int l2_prefetch) {
+                   const int* __restrict__ kv_start, float scale_log2, unsigned long long* trace) {
     constexpr int D = DA_D;
     const int G = H / Hkv;
     const int b = blockIdx.x, hk = blockIdx.y, sp = blockIdx.z;
@@ -154,7 +154,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     }
     __syncthreads();
     pdl_launch_dependents();
-    if (l2_prefetch && warp == 12 && lane == 0) {
+    if (warp == 12 && lane == 0) {
         // Before the dependency resolves: ask L2 for this CTA's K/V chunks.  Only a hint -- nothing is read into the SM, so it does not
         // matter that ctx_len may still hold the previous step's value or that the row the q/k/v projection is appending right now is
         // not there yet (its write lands in the same L2 line; the real loads below come after griddepcontrol.wait).
@@ -444,8 +444,7 @@ int decode_attention(cudaStream_t stream, const bf16* qkv, const bf16* k_cache, 
     int* counters = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(scratch) + partial_bytes(B, H, D, Tmax));
     auto kern = (H / Hkv <= 8) ? decode_attn_kernel<8, ns> : decode_attn_kernel<16, ns>;
     AF3_CHECK_CUDA(launch_kernel(kern, grid, dim3(DA_THREADS), da_smem(ns), stream, mq, mk, mv, scratch, out, counters, H, Hkv, nz,
-                                 ctx_len, kv_start, scale * 1.4426950408889634f, trace_next_slot(),
-                                 [] { const char* e = getenv("AF3_L2_PREFETCH_KV"); return e ? atoi(e) : 1; }()));
+                                 ctx_len, kv_start, scale * 1.4426950408889634f, trace_next_slot()));
     return 0;
 }
 

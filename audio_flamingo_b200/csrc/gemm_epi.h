@@ -17,19 +17,9 @@ struct RopeEpilogue {
     int H, Hkv, Tmax;
 };
 
-// RMSNorm fusion across few-token GEMMs (see GemmArgs in gemm_wgmma.cu): consumer side (norm_w ...) and / or producer side (sumsq_out ...)
-struct NormFusion {
-    const bf16* norm_w;
-    const float* norm_part;
-    int norm_parts, norm_ld;
-    float norm_eps;
-    float* sumsq_out;
-    int sumsq_ld;
-};
-
 int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, void* out, int ldo, int n_tok,
               int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, int res_period,
-              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope, const NormFusion* nf);
+              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope);
 size_t gemm_workspace_bytes();
 
 }  // namespace af3

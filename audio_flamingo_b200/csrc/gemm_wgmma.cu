@@ -52,36 +52,15 @@ struct GemmArgs {
     // by two TMA boxes, and gate_proj.weight / up_proj.weight can simply be VIEWS of the fused matrix (no second copy in HBM)
     int swiglu_up_row0;
     int k_splits;
-    // few-token mode: weight k-blocks BEYOND the shared-memory ring that the producer also requests into L2 before
-    // griddepcontrol.wait (cp.async.bulk.prefetch.tensor): under programmatic dependent launch the CTA can be resident before its
-    // dependency resolves, with HBM idle during the predecessor's tail
-    int l2_prefetch;
-    // cluster_reduce (EXPERIMENT, off by default, see gemm_bf16()): the k_splits CTAs of a tile form a thread-block
-    // cluster and exchange their fp32 partial tiles through distributed shared memory: CTA q of the cluster receives everyone's
-    // partials for ITS slice of the 32 tokens, sums them in split order (deterministic) and runs the fused epilogue for that slice.
-    int cluster_reduce;
     float* ws;      // [tiles][k_splits][BN][128] fp32
     int* counters;  // [tiles], zero on entry, reset to zero by the reducing CTA
     unsigned long long* trace;  // in-graph timeline slot of this launch (common.h) or nullptr
-    // ---- Qwen2RMSNorm fused across two few-token GEMMs of the decode step ([O] Q2M:258-263), removing the norm kernel and its
-    // two dependency hops from the chain:
-    //  * producer (a residual GEMM, transposed epilogue): sumsq_out[token][row tile] = sum over the tile's 128 features of the
-    //    squared bf16 values it just stored;
-    //  * consumer (norm_w != nullptr): rstd[token] = rsqrt(sum over norm_parts partials / K + eps); the consumer warps rewrite every
-    //    activation tile in shared memory as  w[k] * bf16(x[k] * rstd)  (the reference's two roundings) between the TMA completion
-    //    and the wgmma issue.
-    const bf16* norm_w;        // [K] RMSNorm weight of the consumer's input norm, or nullptr
-    const float* norm_part;    // [n_tok][norm_ld] sum-of-squares partials of the input rows, norm_parts (<= 32) used per row
-    int norm_parts, norm_ld;
-    float norm_eps;
-    float* sumsq_out;          // [n_tok][sumsq_ld], entry [tok][row tile], or nullptr
-    int sumsq_ld;
 };
 
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
 constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
 
-template <int BN, int NA, int STAGES, bool SWAP, bool EXP = false>
+template <int BN, int NA, int STAGES, bool SWAP>
 struct GemmCfg {
     static constexpr int R_BYTES = 128 * NA * BK * 2;
     static constexpr int C_BYTES = BN * BK * 2;
@@ -91,11 +70,7 @@ struct GemmCfg {
     static constexpr int ACC_BYTES = 128 * ACC_COLS * 4;
     // normal mode: 4 epilogue warps x 2 buffers x (32 rows x 128 B) staging for the TMA-store epilogue
     // swap mode: one [32 tokens x 128 features] bf16 tile to transpose the accumulator for token-major vector I/O
-    // + (few-token, NA = 1) the landing zone of the cluster split-K reduction: [k_splits][ceil(32 / k_splits)][128] fp32 partial
-    //   slices written by the peer CTAs through distributed shared memory (<= 18.5 KB for 2..8 splits)
-    //   -- experiment instantiations only; the default few-token kernel spends that shared memory on two more ring stages
-    static constexpr int ZONE_BYTES = (SWAP && NA == 1 && EXP) ? 19456 : 0;
-    static constexpr int EPI_STAGE_BYTES = (SWAP ? 32 * 128 * 2 : 4 * 2 * 4096) + ZONE_BYTES;
+    static constexpr int EPI_STAGE_BYTES = SWAP ? 32 * 128 * 2 : 4 * 2 * 4096;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert((2 * STAGES + 8) * 8 + 16 <= 256, "barrier area");
     static_assert(BN == 32 || BN == 128, "BN: wgmma shapes m64n32 / m64n128");
@@ -151,13 +126,11 @@ __device__ __forceinline__ float epi_swiglu(float g, float u) {
 // EW = epilogue warps (4 or 8) among the 8 consumer warps.  With 8 (normal mode, epilogues without a TMA-prefetched residual) two
 // warps share each 32-row quarter of the tile and split its 64-column groups between them: twice the issue slots for epilogue
 // math, which is what bounds short-K GEMMs with expensive epilogues (K = 1280 + GELU: erff per element).
-// EXP: the instantiation that carries the experiments (fused RMSNorm consumer / producer, cluster split-K).  They are compiled OUT
-// of the default kernels so that the few-token instantiations stay small (their one-shot tails run from a cold instruction cache).
-template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW, bool EXP = false>
+template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_c,
             const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
-    using Cfg = GemmCfg<BN, NA, STAGES, SWAP, EXP>;
+    using Cfg = GemmCfg<BN, NA, STAGES, SWAP>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     float* accbuf = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
@@ -170,10 +143,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) trace_mark(a.trace, 0);
-    // experiment switches: compile-time false (dead code) unless EXP
-    [[maybe_unused]] const bool x_norm = EXP && a.norm_w != nullptr;
-    [[maybe_unused]] const bool x_cluster = EXP && a.cluster_reduce != 0;
-    [[maybe_unused]] const bool x_sumsq = EXP && a.sumsq_out != nullptr;
     const int flags = (EPI >= 0) ? EPI : a.flags;
 
     if (warp == 8 && lane == 0) {
@@ -192,11 +161,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
     }
     __syncthreads();
     pdl_launch_dependents();  // the next kernel may start its prologue / weight prefetch behind us
-    if constexpr (SWAP && NA == 1) {
-        // cluster split-K: phase 1 of the cluster barrier only says "this CTA is running" (a peer's shared memory may be written
-        // once it is); everybody arrives here without blocking and waits right before its first remote store / at its end
-        if (x_cluster) cluster_arrive_relaxed();
-    }
 
     const int k_splits = SWAP ? a.k_splits : 1;
     const int num_tiles = a.num_r_tiles * a.num_c_tiles * k_splits;  // work items: (tile, split), split fastest
@@ -228,12 +192,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         for (int na = 0; na < NA; ++na)
                             tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[prefetched], kb * BK,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
-                    }
-                    int pf = a.l2_prefetch;
-                    for (int kb = kb_lo(sp) + prefetched; kb < kb_lo(sp + 1) && pf > 0; ++kb, --pf) {
-#pragma unroll
-                        for (int na = 0; na < NA; ++na)
-                            tma_prefetch_l2_2d(&map_r, kb * BK, a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
                 }
             }
@@ -268,13 +226,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             }
         }
         __syncwarp();
-        if constexpr (SWAP && NA == 1) {
-            if (x_cluster) {   // every thread of the cluster takes part in both phases of the cluster barrier
-                cluster_wait_acquire();
-                cluster_arrive_release();
-                cluster_wait_acquire();
-            }
-        }
     } else {
         // ---- consumer warpgroups: warpgroup wg computes rows [64 wg, 64 wg + 64) of every 128-row block of the row operand with
         //      wgmma (accumulator in registers), hands the finished tile to the epilogue through accbuf, then runs the epilogue
@@ -299,50 +250,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                 for (int na = 0; na < NA; ++na)
 #pragma unroll
                     for (int i = 0; i < BN / 2; ++i) accr[na][i] = 0.f;
-                // fused RMSNorm: rstd of the token whose 16-byte activation chunk this thread rewrites in every k-block
-                [[maybe_unused]] float rstd = 0.f;
-                if constexpr (SWAP && EXP) {
-                    if (x_norm) {
-                        int r0, c0;
-                        tile_coords(t / k_splits, a, r0, c0);
-                        const int tokg = c0 * BN + (threadIdx.x >> 3);
-                        if (tokg < a.n_tok) {
-                            float ss = 0.f;
-                            const float* pp = a.norm_part + static_cast<size_t>(tokg) * a.norm_ld;
-                            for (int p = 0; p < a.norm_parts; ++p) ss += __ldcg(pp + p);
-                            rstd = rsqrtf(ss / static_cast<float>(a.K) + a.norm_eps);
-                        }
-                    }
-                }
                 int prev = -1;
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(&full[stage], phase);
-                    uint8_t* sRp = smem + stage * Cfg::STAGE_BYTES;
-                    if constexpr (SWAP && EXP) {
-                        if (x_norm) {
-                            // fused RMSNorm of the activation tile [32 tokens][64] (128B-swizzled rows): thread = (token, 16-byte chunk);
-                            // w[k] * bf16(x[k] * rstd): the product of two bf16 values rounded to bf16 is what HFMA2.BF16 computes
-                            const int tok = threadIdx.x >> 3, j = threadIdx.x & 7;
-                            uint4* px = reinterpret_cast<uint4*>(sRp + Cfg::R_BYTES + tok * 128 + ((j ^ (tok & 7)) << 4));
-                            const uint4 wq = __ldg(reinterpret_cast<const uint4*>(a.norm_w) + kb * 8 + j);
-                            const uint4 xv = *px;
-                            const __nv_bfloat162* xh = reinterpret_cast<const __nv_bfloat162*>(&xv);
-                            const __nv_bfloat162* wh = reinterpret_cast<const __nv_bfloat162*>(&wq);
-                            const __nv_bfloat162 zero2 = __floats2bfloat162_rn(0.f, 0.f);
-                            uint32_t o[4];
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float2 xf2 = __bfloat1622float2(xh[e]);
-                                const __nv_bfloat162 xn = __floats2bfloat162_rn(xf2.x * rstd, xf2.y * rstd);
-                                const __nv_bfloat162 y = __hfma2(wh[e], xn, zero2);
-                                o[e] = *reinterpret_cast<const uint32_t*>(&y);
-                            }
-                            *px = make_uint4(o[0], o[1], o[2], o[3]);
-                            fence_proxy_async_smem();
-                            asm volatile("bar.sync 3, 256;" ::: "memory");
-                        }
-                    }
-                    const uint32_t sR = smem_u32(sRp);
+                    const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
                     const uint32_t sC = sR + Cfg::R_BYTES;
 #pragma unroll
                     for (int na = 0; na < NA; ++na) fence_regs(accr[na]);
@@ -635,37 +546,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                     uint32_t v[32], u[32];
                     acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, ch * 32, v);
                     if constexpr (NA == 2) acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, BN + ch * 32, u);
-                    [[maybe_unused]] int tok_lo = 0, tok_hi = 0x7fffffff;   // tokens this CTA finishes (cluster reduce: its slice)
                     if constexpr (NA == 1 && BN == 32) {
-                        if (k_splits > 1 && x_cluster) {
-                            const int ks = k_splits, rank = t % k_splits;       // == %cluster_ctarank (consecutive CTAs form a cluster)
-                            const int tokmax = (32 + ks - 1) / ks;
-                            float* zone = reinterpret_cast<float*>(epi_stage + 32 * 128 * 2);   // [ks][tokmax][128]
-                            const uint32_t zone_cta = smem_u32(zone);
-                            cluster_wait_acquire();   // phase 1: every CTA of the cluster is running
-                            // rank q owns tokens [q * 32 / ks, (q + 1) * 32 / ks): send it this CTA's partials of those tokens
-#pragma unroll 1
-                            for (int q = 0; q < ks; ++q) {
-                                const int lo_q = (q * 32) / ks, hi_q = ((q + 1) * 32) / ks;
-                                const uint32_t dst = mapa_shared(zone_cta, q) + (((rank * tokmax - lo_q) * 128 + row_in_tile) << 2);
-#pragma unroll
-                                for (int j = 0; j < 32; ++j)
-                                    if (j >= lo_q && j < hi_q) st_cluster_f32(dst + j * 512, __uint_as_float(v[j]));
-                            }
-                            cluster_arrive_release();
-                            cluster_wait_acquire();
-                            const int lo = (rank * 32) / ks, hi = ((rank + 1) * 32) / ks;
-                            tok_lo = c * BN + lo;
-                            tok_hi = c * BN + hi;
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                if (j >= lo && j < hi) {
-                                    float sum = 0.f;
-                                    for (int s2 = 0; s2 < ks; ++s2) sum += zone[(s2 * tokmax + (j - lo)) * 128 + row_in_tile];   // split order
-                                    v[j] = __float_as_uint(sum);
-                                }
-                            }
-                        } else if (k_splits > 1) {
+                        if (k_splits > 1) {
                             // publish this split's partial tile: ws[tile][split][col][row] (row fastest: coalesced)
                             const int tile = t / k_splits, sp = t % k_splits;
                             float* wt = a.ws + (static_cast<size_t>(tile) * k_splits) * (BN * 128);
@@ -730,8 +612,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                             const int et = threadIdx.x;             // 0..127 within the epilogue warps
                             const int tok = tok0 + (et >> 2);
                             const int f0 = r * 128 + (et & 3) * 32;      // first of this thread's 32 features
-                            const bool mine = tok >= tok_lo && tok < tok_hi;
-                            if ((flags & EPI_ROPE) && tok < a.n_tok && mine) {
+                            if ((flags & EPI_ROPE) && tok < a.n_tok) {
                                 // tile r = head r of the fused projection: [0,H) query, [H,H+Hkv) key, then value heads
                                 const int head = r, q4 = et & 3;
                                 const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + q4 * 32);
@@ -773,10 +654,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 #pragma unroll
                                     for (int g4 = 0; g4 < 4; ++g4) reinterpret_cast<uint4*>(op)[g4] = tp[g4];
                                 }
-                            } else if (!(flags & EPI_ROPE) && tok < a.n_tok && mine) {
+                            } else if (!(flags & EPI_ROPE) && tok < a.n_tok) {
                                 const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + (et & 3) * 32);
                                 bf16* op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                                float ssq = 0.f;   // sum of squares of the bf16 values stored below (fused RMSNorm producer)
                                 uint4 rv[4];
                                 if (flags & EPI_RESID) {
                                     if constexpr (NA == 1) {
@@ -807,24 +687,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                                             yv = make_uint4(o4[0], o4[1], o4[2], o4[3]);
                                         }
                                         reinterpret_cast<uint4*>(op)[g4] = yv;
-                                        if (x_sumsq) {
-                                            const __nv_bfloat162* yh = reinterpret_cast<const __nv_bfloat162*>(&yv);
-#pragma unroll
-                                            for (int e = 0; e < 4; ++e) {
-                                                const float2 yf = __bfloat1622float2(yh[e]);
-                                                ssq = fmaf(yf.x, yf.x, ssq);
-                                                ssq = fmaf(yf.y, yf.y, ssq);
-                                            }
-                                        }
                                     }
-                                }
-                                if (x_sumsq) {
-                                    // the four lanes et % 4 = 0..3 hold the token's 4 x 32 features of this row tile (same warp, same
-                                    // branch: tok is uniform over them); fixed order -> deterministic
-                                    const unsigned grp = 0xFu << (lane & 28);
-                                    ssq += __shfl_xor_sync(grp, ssq, 1);
-                                    ssq += __shfl_xor_sync(grp, ssq, 2);
-                                    if ((et & 3) == 0) a.sumsq_out[static_cast<size_t>(tok) * a.sumsq_ld + r] = ssq;
                                 }
                             }
                             asm volatile("bar.sync 2, 128;" ::: "memory");  // tile may be rewritten by the next work item
@@ -861,13 +724,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                 }
             }
         }
-        if constexpr (SWAP && NA == 1) {
-            if (x_cluster && !epi_warp) {
-                cluster_wait_acquire();
-                cluster_arrive_release();
-                cluster_wait_acquire();
-            }
-        }
     }
 
     if (!SWAP && warp < EW && lane == 0) bulk_wait_read<0>();  // staged tiles must be read out before smem goes away
@@ -875,49 +731,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
-template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW = 4, bool EXP = false>
+template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW = 4>
 static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMap& mo, const CUtensorMap& mres,
                   const GemmArgs& a, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, NA, STAGES, SWAP, EXP>;
-    auto kern = gemm_kernel<BN, NA, STAGES, SWAP, EPI, EW, EXP>;
+    using Cfg = GemmCfg<BN, NA, STAGES, SWAP>;
+    auto kern = gemm_kernel<BN, NA, STAGES, SWAP, EPI, EW>;
     static DeviceOnce once;
     if (once.first()) {
         AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    }
-    if constexpr (SWAP && NA == 1 && EXP) {
-        if (a.cluster_reduce && a.k_splits > 1) {
-            // cluster split-K: the largest split count <= the requested one for which all tiles' clusters are co-resident
-            // (a cluster needs k_splits free SMs inside ONE GPC; the answer is cached per device and cluster size)
-            static int cache[128][9];
-            static bool cache_init = false;
-            if (!cache_init) {
-                for (auto& row : cache)
-                    for (int& v : row) v = -1;
-                cache_init = true;
-            }
-            const int dev = current_device() & 127;
-            const int base_tiles = a.num_r_tiles * a.num_c_tiles;
-            int ks = a.k_splits > 8 ? 8 : a.k_splits;
-            for (; ks >= 2; --ks) {
-                if (cache[dev][ks] < 0) cache[dev][ks] = max_active_clusters(kern, dim3(GEMM_THREADS), Cfg::SMEM_BYTES, ks);
-                if (cache[dev][ks] >= base_tiles && base_tiles * ks <= sm_count()) break;
-            }
-            if (ks >= 2) {
-                GemmArgs b = a;
-                b.k_splits = ks;
-                AF3_CHECK_CUDA(launch_kernel_cluster(kern, dim3(base_tiles * ks), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, ks, mr, mc, mo,
-                                                     mres, b));
-                return 0;
-            }
-            // no cluster size fits: global-memory reduction (below) when a workspace was given, else no split
-            GemmArgs b = a;
-            b.cluster_reduce = 0;
-            if (!b.ws) b.k_splits = 1;
-            const int tiles_b = base_tiles * b.k_splits;
-            AF3_CHECK_CUDA(launch_kernel(kern, dim3(tiles_b < sm_count() ? tiles_b : sm_count()), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, mr,
-                                         mc, mo, mres, b));
-            return 0;
-        }
     }
     const int tiles = a.num_r_tiles * a.num_c_tiles * (SWAP && a.k_splits > 1 ? a.k_splits : 1);
     const int grid = tiles < sm_count() ? tiles : sm_count();
@@ -928,13 +749,12 @@ static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const CUtens
 // Host entry.  x: [n_tok, K] bf16 (pitch ldx), w: [n_rows_w, K] bf16 (pitch ldw) where n_rows_w = n_feat, or the
 // gate/up-interleaved 2*ceil(n_feat/128)*128 rows when EPI_SWIGLU.  out: [n_tok, n_feat] (pitch ldo).
 // compile-time epilogue specialisations for the flag sets the AF3 path uses; anything else -> generic (-1)
-template <int BN, int NA, int STAGES, bool SWAP, bool EXP = false>
+template <int BN, int NA, int STAGES, bool SWAP>
 static int launch(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMap& mo, const CUtensorMap& mres,
                   const GemmArgs& a, cudaStream_t stream) {
-    // few-token kernels: the experiments (RMSNorm fusion, cluster split-K) live in their own instantiations (EXP)
 #define AF3_EPI_CASE(F) \
     case (F):           \
-        return launch_epi<BN, NA, STAGES, SWAP, (F), 4, EXP>(mr, mc, mo, mres, a, stream);
+        return launch_epi<BN, NA, STAGES, SWAP, (F)>(mr, mc, mo, mres, a, stream);
     if constexpr (!SWAP) {
         // 8 epilogue warps where the epilogue (not the MMA) bounds the tile: TMA-store path without a TMA residual
         if (a.tma_epi && !((a.flags & EPI_RESID) && a.res_period == 0)) {
@@ -968,14 +788,14 @@ static int launch(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMa
         }
     }
 #undef AF3_EPI_CASE
-    return launch_epi<BN, NA, STAGES, SWAP, -1, 4, EXP>(mr, mc, mo, mres, a, stream);
+    return launch_epi<BN, NA, STAGES, SWAP, -1>(mr, mc, mo, mres, a, stream);
 }
 
 size_t gemm_workspace_bytes() { return (8u << 20) + 4096 * sizeof(int); }
 
 int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, void* out, int ldo, int n_tok,
               int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, int res_period,
-              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope, const NormFusion* nf) {
+              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope) {
     AF3_REQUIRE(n_tok > 0 && n_feat > 0 && K > 0, "gemm: empty problem");
     AF3_REQUIRE((K % 8) == 0 && (ldx % 8) == 0 && (ldw % 8) == 0, "gemm: K and pitches must be multiples of 8");
     AF3_REQUIRE(!(flags & EPI_BIAS) || bias, "gemm: bias flag without pointer");
@@ -999,27 +819,6 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
     a.swiglu_up_row0 = concat ? n_feat : 0;
     a.k_splits = 1;
     a.trace = trace_next_slot();
-    if (nf) {
-        AF3_REQUIRE(n_tok <= 64, "gemm: RMSNorm fusion exists for the few-token (decode) GEMMs only");
-        if (nf->norm_w) {
-            AF3_REQUIRE(nf->norm_part && nf->norm_parts > 0 && nf->norm_parts <= 32 && nf->norm_ld >= 32 && nf->norm_ld % 4 == 0 &&
-                            (reinterpret_cast<uintptr_t>(nf->norm_part) & 15) == 0,
-                        "gemm: fused RMSNorm needs <= 32 sum-of-squares partials per token in 16-byte aligned rows of >= 32 floats");
-            AF3_REQUIRE(K % 64 == 0 && (reinterpret_cast<uintptr_t>(nf->norm_w) & 15) == 0, "gemm: fused RMSNorm needs K % 64 == 0 and a 16-byte aligned weight");
-            a.norm_w = nf->norm_w;
-            a.norm_part = nf->norm_part;
-            a.norm_parts = nf->norm_parts;
-            a.norm_ld = nf->norm_ld;
-            a.norm_eps = nf->norm_eps;
-        }
-        if (nf->sumsq_out) {
-            AF3_REQUIRE(nf->sumsq_ld >= ceil_div(n_feat, 128) && !(flags & (EPI_F32OUT | EPI_SWIGLU | EPI_ROPE)) && (ldo % 8) == 0 && res_period == 0 &&
-                            (!(flags & EPI_RESID) || (ld_res % 8) == 0),
-                        "gemm: sum-of-squares output needs the token-major bf16 epilogue");
-            a.sumsq_out = nf->sumsq_out;
-            a.sumsq_ld = nf->sumsq_ld;
-        }
-    }
     if (flags & EPI_ROPE) {
         AF3_REQUIRE(rope && rope->cs && rope->k_cache && rope->v_cache && rope->pos, "gemm: EPI_ROPE needs the rope arguments");
         AF3_REQUIRE(n_tok <= 64 && n_feat == (rope->H + 2 * rope->Hkv) * 128 && (ldo % 8) == 0 && !(flags & (EPI_RESID | EPI_F32OUT | EPI_SWIGLU)),
@@ -1065,7 +864,6 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
     constexpr int BN = 32;
     a.R = w_rows;
     a.C = n_tok;
-    a.l2_prefetch = [&] { const char* e = getenv(swiglu ? "AF3_L2_PREFETCH_GU" : "AF3_L2_PREFETCH"); return e ? atoi(e) : 0; }();
     a.num_c_tiles = ceil_div(n_tok, BN);
     a.group_r = 1;
     if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, 128)) return e;
@@ -1074,7 +872,7 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
     // allows next to the accumulator tile: the weight streams of a few-token GEMM are latency-bound on the bytes in flight per SM.
     if (swiglu) {
         a.num_r_tiles = ceil_div(w_rows, 256);
-        return (a.norm_w || a.sumsq_out) ? launch<BN, 2, 5, true, true>(mw, mx, mw, mw, a, stream) : launch<BN, 2, 5, true>(mw, mx, mw, mw, a, stream);
+        return launch<BN, 2, 5, true>(mw, mx, mw, mw, a, stream);
     }
     a.num_r_tiles = ceil_div(w_rows, 128);
     // split-K when the tile grid cannot fill the GPU and a (zero-initialised) workspace was supplied
@@ -1091,18 +889,9 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
             a.k_splits = s;
             a.ws = reinterpret_cast<float*>(workspace);
             a.counters = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(workspace) + (8u << 20));
-            // opt-in (AF3_CLUSTER_REDUCE=1): reduce through distributed shared memory inside a thread-block cluster when the
-            // token-major bf16 epilogue applies, instead of through the global-memory workspace.  A cluster can only become resident
-            // when k_splits SMs of one GPC are free, which costs the early (pre-dependency) weight prefetch under programmatic
-            // dependent launch.
-            const char* e = getenv("AF3_CLUSTER_REDUCE");
-            const bool transposed_epi = !(flags & EPI_F32OUT) && (ldo % 8) == 0 && (!(flags & EPI_RESID) || ((ld_res % 8) == 0 && res_period == 0));
-            a.cluster_reduce = ((e && e[0] == '1') && transposed_epi) ? 1 : 0;
         }
     }
-    // ring depth: 10 x 20 KB = 200 KB in flight per SM (the few-token streams are latency-bound on bytes in flight); the experiment
-    // instantiations keep 8 stages next to their 19 KB exchange zone
-    if (a.norm_w || a.sumsq_out || a.cluster_reduce) return launch<BN, 1, 8, true, true>(mw, mx, mw, mw, a, stream);
+    // ring depth: 10 x 20 KB = 200 KB in flight per SM (the few-token streams are latency-bound on bytes in flight)
     return launch<BN, 1, 10, true>(mw, mx, mw, mw, a, stream);
 }
 

@@ -1,5 +1,5 @@
 // Thin inline-PTX wrappers for the sm_90a primitives the AF3 hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait), clusters and fences.
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) and fences.
 // Hand-written for this repo; every wrapper is a single PTX instruction (or a spin loop on one).
 #pragma once
 #include <cuda_bf16.h>
@@ -79,26 +79,6 @@ __device__ __forceinline__ void trace_mark(unsigned long long* slot, int mark) {
     }
 }
 
-// ---------------------------------------------------------------- thread-block clusters / distributed shared memory
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// shared::cta address of this CTA -> shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t cta_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(cta_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void st_cluster_f32(uint32_t cluster_addr, float v) {
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
-}
-// cluster-wide barrier, split: every thread of every CTA of the cluster arrives once and waits once per phase
-__device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-
 // ---------------------------------------------------------------- proxy fences
 // generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() {
@@ -115,10 +95,7 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* map, uin
         ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// L2-only prefetch of the box a later tma_load_2d will fetch (no shared memory, no barrier)
-__device__ __forceinline__ void tma_prefetch_l2_2d(const void* map, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
-}
+// L2-only prefetch of the box a later tma_load_3d will fetch (no shared memory, no barrier)
 __device__ __forceinline__ void tma_prefetch_l2_3d(const void* map, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }

@@ -353,18 +353,8 @@ class Qwen2ForCausalLM(nn.Module):
         pos0 = cache.length
         rope_cs = None
         fused_qkv = decode and B <= 64  # few-token ("swapped") GEMM with RoPE + KV append in its epilogue
-        # Decode step with RMSNorm fused ACROSS the GEMMs (include/af3b200.h af3_gemm_fusion): the residual GEMMs (o, down) emit the
-        # per-row-tile sums of squares of the rows they store, the next q/k/v / gate-up GEMM normalises its activation tiles in shared
-        # memory; 55 of the 57 norm launches of a step disappear.  OPT-IN (AF3_FUSE_NORM=1): parity-clean, but not shown to be faster
-        # than the chain with stand-alone norm kernels: the few-token streams are latency-bound on ring depth, and a stage that waits
-        # for its activation tile to be rewritten is a stage not in flight.
-        fuse_norm = fused_qkv and self.hid % 64 == 0 and self.hid <= 4096 and os.environ.get("AF3_FUSE_NORM", "0") == "1"
-        n_parts = -(-self.hid // 128)
         if fused_qkv:
             rope_cs = ops.rope_table(B, D, cache.pos_dev, cache.kv_start, self._inv_freq)
-        ss = ss_attn = ss_mlp = None   # ss: partials describing the CURRENT residual stream h (None -> stand-alone norm kernel)
-        if fuse_norm:
-            ss_attn, ss_mlp = ops.sumsq_buffer(B, h.device), ops.sumsq_buffer(B, h.device)
         y = None
         for li, (l, (wqkv, bqkv, wgu)) in enumerate(zip(self.model.layers, self._packed)):
             kc, vc = cache.k[li], cache.v[li]
@@ -372,12 +362,8 @@ class Qwen2ForCausalLM(nn.Module):
             if decode:
                 if fused_qkv:
                     # q/k/v projection with RoPE + KV append in the GEMM epilogue (rope table: once per step, above)
-                    if ss is not None:
-                        qkv = ops.qkv_rope_linear(h, wqkv, bqkv, kc, vc, H=H, Hkv=Hkv, D=D, rope_cs=rope_cs, pos_dev=cache.pos_dev,
-                                                  norm=(l.input_layernorm.weight, ss, n_parts, self.eps))
-                    else:
-                        y = ops.rmsnorm(h, l.input_layernorm.weight, self.eps, out=y)
-                        qkv = ops.qkv_rope_linear(y, wqkv, bqkv, kc, vc, H=H, Hkv=Hkv, D=D, rope_cs=rope_cs, pos_dev=cache.pos_dev)
+                    y = ops.rmsnorm(h, l.input_layernorm.weight, self.eps, out=y)
+                    qkv = ops.qkv_rope_linear(y, wqkv, bqkv, kc, vc, H=H, Hkv=Hkv, D=D, rope_cs=rope_cs, pos_dev=cache.pos_dev)
                 else:
                     # more than 64 sequences per GPU: token-major tensor-core GEMM + the stand-alone RoPE / append kernel reading
                     # the slot from device memory (graph replay)
@@ -395,17 +381,10 @@ class Qwen2ForCausalLM(nn.Module):
                 ops.attention(qkv, kc, vc, a.view(B, T, H * D), B=B, H=H, Hkv=Hkv, D=D, Tq=T, Tk=pos0 + T, scale=D ** -0.5,
                               causal=True, kv_layout=1, Tk_pitch=cache.Tmax, ldq=(H + 2 * Hkv) * D, ldk=D,
                               kv_start=cache.kv_start)
-            if fuse_norm:
-                ops.linear(a, l.self_attn.o_proj.weight, resid=h, out=h, sumsq_out=ss_attn)
-                g = ops.swiglu_linear(h, wgu, self.inter, norm=(l.post_attention_layernorm.weight, ss_attn, n_parts, self.eps),
-                                      concat=self._swiglu_concat)
-                ops.linear(g, l.mlp.down_proj.weight, resid=h, out=h, sumsq_out=ss_mlp)
-                ss = ss_mlp
-            else:
-                ops.linear(a, l.self_attn.o_proj.weight, resid=h, out=h)
-                y = ops.rmsnorm(h, l.post_attention_layernorm.weight, self.eps, out=y)
-                g = ops.swiglu_linear(y, wgu, self.inter, concat=self._swiglu_concat)
-                ops.linear(g, l.mlp.down_proj.weight, resid=h, out=h)
+            ops.linear(a, l.self_attn.o_proj.weight, resid=h, out=h)
+            y = ops.rmsnorm(h, l.post_attention_layernorm.weight, self.eps, out=y)
+            g = ops.swiglu_linear(y, wgu, self.inter, concat=self._swiglu_concat)
+            ops.linear(g, l.mlp.down_proj.weight, resid=h, out=h)
         return h
 
     def _head(self, h, row_idx=None):
@@ -746,8 +725,8 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             Tmax = AF3KVCache.bucket(S + max_new_tokens)
             # the captured graph holds raw addresses: key it on the weight storages too, so a re-pack (load_reference_state_dict) or
             # a move (.to()) can never leave a stale graph replaying against freed memory
-            key = (B, Tmax, use_graph, os.environ.get("AF3_PDL", "1") != "0", os.environ.get("AF3_FUSE_NORM", "0") == "1",
-                   "|".join(os.environ.get(k, "") for k in ("AF3_L2_PREFETCH", "AF3_L2_PREFETCH_GU", "AF3_L2_PREFETCH_KV")), str(dev), lm.lm_head.weight.data_ptr(), lm._packed[0][0].data_ptr(), lm._packed[-1][2].data_ptr())
+            key = (B, Tmax, use_graph, os.environ.get("AF3_PDL", "1") != "0", str(dev), lm.lm_head.weight.data_ptr(),
+                   lm._packed[0][0].data_ptr(), lm._packed[-1][2].data_ptr())
             st = self._decode_state
             if st is not None and st["key"] == key:
                 cache, step_fn = st["cache"], st["step"]       # same buffers -> the captured graph is valid as it stands

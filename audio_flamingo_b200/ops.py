@@ -5,7 +5,6 @@ through ctypes.  All arithmetic happens in libaf3b200.so; nothing here falls bac
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 
 import numpy as np
@@ -81,31 +80,8 @@ def gemm_workspace(device):
     return ws
 
 
-def _fusion(norm, sumsq_out):
-    """ctypes af3_gemm_fusion or None.  norm = (weight bf16 [K], partials fp32 [n_tok, >= 32], number of partials per row, eps);
-    sumsq_out fp32 [n_tok, >= 32] (see sumsq_buffer)."""
-    if norm is None and sumsq_out is None:
-        return None
-    f = _lib.GemmFusion()
-    if norm is not None:
-        wn, part, nparts, eps = norm
-        _req(wn, bf16, "norm weight"), _req(part, torch.float32, "norm partials")
-        f.norm_weight, f.norm_sumsq, f.norm_parts, f.norm_ld, f.norm_eps = ptr(wn), ptr(part), int(nparts), part.stride(0), float(eps)
-    if sumsq_out is not None:
-        _req(sumsq_out, torch.float32, "sumsq_out")
-        f.sumsq_out, f.sumsq_ld = ptr(sumsq_out), sumsq_out.stride(0)
-    return f
-
-
-def sumsq_buffer(n_tok, device):
-    """fp32 [n_tok, 32]: per token, one sum of squares per 128-feature row tile of what a residual GEMM stores (up to 32 tiles =
-    4096 features), consumed by the next GEMM's fused RMSNorm."""
-    return torch.empty((n_tok, 32), device=device, dtype=torch.float32)
-
-
-def linear(x, w, bias=None, *, gelu=False, resid=None, res_period=0, out=None, out_f32=False, norm=None, sumsq_out=None):
-    """out = epi(x @ w.T); x [n_tok, K] bf16, w [n_feat, K] bf16 (nn.Linear layout).
-    norm / sumsq_out: RMSNorm fusion across few-token GEMMs (include/af3b200.h af3_gemm_fusion)."""
+def linear(x, w, bias=None, *, gelu=False, resid=None, res_period=0, out=None, out_f32=False):
+    """out = epi(x @ w.T); x [n_tok, K] bf16, w [n_feat, K] bf16 (nn.Linear layout)."""
     lib = _lib.load()
     _req(x, bf16, "x"), _req(w, bf16, "w")
     n_tok, K = x.shape
@@ -124,12 +100,11 @@ def linear(x, w, bias=None, *, gelu=False, resid=None, res_period=0, out=None, o
     if out is None:
         out = torch.empty((n_tok, n_feat), device=x.device, dtype=torch.float32 if out_f32 else bf16)
     ws = gemm_workspace(x.device) if n_tok <= 64 else None
-    fus = _fusion(norm, sumsq_out)
     with _Timed(("gemm", n_tok, n_feat, K, flags)):
         check(
-            lib.af3_gemm_bf16_fused(stream_ptr(), ptr(x), x.stride(0), ptr(w), w.stride(0), ptr(out), out.stride(0), n_tok, n_feat,
-                                    K, flags, ptr(bias), ptr(resid), resid.stride(0) if resid is not None else 0, res_period,
-                                    ptr(ws), ws.numel() if ws is not None else 0, C.byref(fus) if fus is not None else None),
+            lib.af3_gemm_bf16_ws(stream_ptr(), ptr(x), x.stride(0), ptr(w), w.stride(0), ptr(out), out.stride(0), n_tok, n_feat,
+                                 K, flags, ptr(bias), ptr(resid), resid.stride(0) if resid is not None else 0, res_period,
+                                 ptr(ws), ws.numel() if ws is not None else 0),
             "af3_gemm_bf16",
         )
     _count(1)
@@ -146,20 +121,18 @@ def pack_gate_up(gate, up):
     return packed
 
 
-def swiglu_linear(x, w_packed, n_feat, out=None, norm=None, concat=False):
+def swiglu_linear(x, w_packed, n_feat, out=None, concat=False):
     """out = silu(x @ gate.T) * (x @ up.T).  w_packed: from pack_gate_up (128-row interleave), or with concat=True the plain
-    [gate; up] concatenation (n_feat % 128 == 0).  norm: fused RMSNorm of x (few-token mode)."""
+    [gate; up] concatenation (n_feat % 128 == 0)."""
     lib = _lib.load()
     _req(x, bf16, "x"), _req(w_packed, bf16, "w_packed")
     n_tok, K = x.shape
     if out is None:
         out = torch.empty((n_tok, n_feat), device=x.device, dtype=bf16)
-    fus = _fusion(norm, None)
     with _Timed(("gemm", n_tok, n_feat, K, EPI_SWIGLU)):
         check(
-            lib.af3_gemm_bf16_fused(stream_ptr(), ptr(x), x.stride(0), ptr(w_packed), w_packed.stride(0), ptr(out), out.stride(0),
-                                    n_tok, n_feat, K, EPI_SWIGLU | (EPI_SWIGLU_CONCAT if concat else 0), None, None, 0, 0, None, 0,
-                                    C.byref(fus) if fus is not None else None),
+            lib.af3_gemm_bf16_ws(stream_ptr(), ptr(x), x.stride(0), ptr(w_packed), w_packed.stride(0), ptr(out), out.stride(0),
+                                 n_tok, n_feat, K, EPI_SWIGLU | (EPI_SWIGLU_CONCAT if concat else 0), None, None, 0, 0, None, 0),
             "af3_gemm_bf16(swiglu)",
         )
     _count(1)
@@ -333,7 +306,7 @@ def rope_table(B, D, pos_dev, kv_start, inv_freq, out=None):
     return out
 
 
-def qkv_rope_linear(x, w, bias, k_cache, v_cache, *, H, Hkv, D, rope_cs, pos_dev, out=None, norm=None):
+def qkv_rope_linear(x, w, bias, k_cache, v_cache, *, H, Hkv, D, rope_cs, pos_dev, out=None):
     """Decode-step q/k/v projection with RoPE + KV append fused into the GEMM epilogue.  Returns the [n_tok, (H+2Hkv)*D]
     buffer whose first H*D columns hold the rotated queries (k / v go straight into the caches)."""
     lib = _lib.load()
@@ -343,12 +316,10 @@ def qkv_rope_linear(x, w, bias, k_cache, v_cache, *, H, Hkv, D, rope_cs, pos_dev
         out = torch.empty((n_tok, (H + 2 * Hkv) * D), device=x.device, dtype=bf16)
     ws = gemm_workspace(x.device)
     Tmax = k_cache.shape[2]
-    fus = _fusion(norm, None)
     with _Timed(("gemm", n_tok, (H + 2 * Hkv) * D, K, EPI_BIAS | 32)):
         check(
             lib.af3_gemm_qkv_rope(stream_ptr(), ptr(x), x.stride(0), ptr(w), w.stride(0), ptr(bias), ptr(out), out.stride(0), n_tok, K,
-                                  H, Hkv, D, ptr(rope_cs), ptr(k_cache), ptr(v_cache), Tmax, ptr(pos_dev), ptr(ws), ws.numel(),
-                                  C.byref(fus) if fus is not None else None),
+                                  H, Hkv, D, ptr(rope_cs), ptr(k_cache), ptr(v_cache), Tmax, ptr(pos_dev), ptr(ws), ws.numel()),
             "af3_gemm_qkv_rope",
         )
     _count(1)

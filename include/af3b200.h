@@ -134,36 +134,12 @@ int af3_gated_residual(void* stream, const void* resid, const void* y, const voi
 /* Decode-step fusion of the q/k/v projection with RoPE and the KV append (Q2M:199-215 + CACHE:119-120 in one kernel):
  * out rows get the ROTATED query heads (columns [0, H*D)); rotated keys and the values go straight into the caches at
  * slot *pos_dev.  rope_cs [n_tok][D/2][2] fp32 from af3_rope_table (once per step, shared by all layers).
- * n_tok <= 64, D = 128, bias required (Qwen2 q/k/v have biases). */
-int af3_rope_table(void* stream, float* rope_cs, int B, int D, const int* pos_dev, const int* kv_start,
-                   const float* inv_freq);
-
-/* Qwen2RMSNorm ([O] Q2M:258-263) fused ACROSS two few-token (n_tok <= 64) GEMMs of the decode step, so that the norm kernel and
- * its two dependency hops leave the step's kernel chain:
- *   producer side (a GEMM with the bf16 token-major epilogue, typically the residual o / down projection): sumsq_out
- *     [n_tok][sumsq_ld] receives, per token, one sum of squares per 128-feature row tile (entry [tok][tile]) of the bf16
- *     values the GEMM stored;
- *   consumer side (the next q/k/v or gate/up projection): x is the UN-normalised residual stream; with norm_weight [K] bf16 and the
- *     producer's partials (norm_sumsq [n_tok][norm_ld], the first norm_parts <= 32 entries of a row are summed, norm_ld >= 32 and a
- *     multiple of 4, rows 16-byte aligned) the kernel computes rstd = rsqrt(sum / K + eps) per token and feeds the tensor cores
- *     norm_weight[k] * bf16(x[k] * rstd)  -- the reference's two roundings -- instead of x.
- * Either side may be left out (NULL pointers).  K % 64 == 0.  Deterministic (fixed summation order). */
-typedef struct af3_gemm_fusion {
-    const void* norm_weight; /* bf16 [K] or NULL */
-    const float* norm_sumsq; /* [n_tok][norm_ld], norm_parts used per row */
-    int norm_parts, norm_ld;
-    float norm_eps;
-    float* sumsq_out;        /* [n_tok][sumsq_ld >= ceil(n_feat/128)] or NULL */
-    int sumsq_ld;
-} af3_gemm_fusion;
-/* af3_gemm_bf16_ws plus the fusion descriptor (NULL = plain). */
-int af3_gemm_bf16_fused(void* stream, const void* x, int ldx, const void* w, int ldw, void* out, int ldo, int n_tok,
-                        int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res, int res_period,
-                        void* workspace, size_t workspace_bytes, const af3_gemm_fusion* fusion);
-
+ * n_tok <= 64, D = 128, bias required (Qwen2 q/k/v have biases).  (ABI v4: RMSNorm fusion removed) */
 int af3_gemm_qkv_rope(void* stream, const void* x, int ldx, const void* w, int ldw, const void* bias, void* q_out, int ldo,
                       int n_tok, int K, int H, int Hkv, int D, const float* rope_cs, void* k_cache, void* v_cache, int Tmax,
-                      const int* pos_dev, void* workspace, size_t workspace_bytes, const af3_gemm_fusion* fusion /* consumer side or NULL */);
+                      const int* pos_dev, void* workspace, size_t workspace_bytes);
+int af3_rope_table(void* stream, float* rope_cs, int B, int D, const int* pos_dev, const int* kv_start,
+                   const float* inv_freq);
 
 /* Single-token attention over the KV cache (decode step; SDPA:40-104 with q_len = 1).  ctx_len is read from device
  * memory so the launch can live in a CUDA graph.  q at qkv (packed [B, (H+2Hkv)*D]); out [B, H*D].

@@ -8,7 +8,7 @@ in a CUDA graph WITH the trace slots baked in, replays it, and reads back per-CT
 Output: JSON (one record per launch + per-kind aggregates) and a markdown summary.
 
     python profiles/decode_timeline.py --out /tmp/decode_timeline --tag base
-Environment knobs under test are simply inherited (AF3_PDL, AF3_FUSE_NORM, AF3_L2_PREFETCH*, AF3_KSPLIT, ...).
+Environment knobs under test are simply inherited (AF3_PDL, AF3_KSPLIT, ...).
 """
 from __future__ import annotations
 

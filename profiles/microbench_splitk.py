@@ -1,6 +1,7 @@
 """Few-token (decode) GEMM: time per launch and its split into weight streaming vs reduction/epilogue tail, as a function of the
-number of K splits (the split-K tail: last accumulator ready -> last CTA exit); this sweep measures (a) how the tail scales with
-the split count and (b) whether fewer CTAs still pull the weights at HBM speed.
+number of K splits, whose partial tiles are reduced through global memory (the split-K tail: last accumulator ready -> last CTA
+exit); this sweep measures (a) how the tail scales with the split count and (b) whether fewer CTAs still pull the weights at HBM
+speed.
     python profiles/microbench_splitk.py > splitk.json
 us per launch: CUDA events around a graph of 48 back-to-back launches (no PDL), weights rotated over 12 copies so every launch
 streams from HBM.  stream / tail: library trace (%globaltimer) of 12 eager launches, medians."""
@@ -36,10 +37,7 @@ def run_shape(name, N, K, mode, copies=12, iters=48):
             ops.linear(x, w, resid=out, out=out)
 
     rows = []
-    for cluster, ks in [(c, k) for c in ("1", "0") for k in (1, 2, 3, 4, 5, 6, 8)]:
-        if cluster == "0" and ks == 1:
-            continue
-        os.environ["AF3_CLUSTER_REDUCE"] = cluster   # 1: partials through distributed shared memory (cluster), 0: through L2 + counters
+    for ks in (1, 2, 3, 4, 5, 6, 8):
         os.environ["AF3_KSPLIT"] = str(ks)
         for i in range(4):
             run(i)
@@ -73,11 +71,10 @@ def run_shape(name, N, K, mode, copies=12, iters=48):
             t_wait = int(m[live, 1][m[live, 1] > 0].min())
             stream.append((int(m[live, 2].max()) - t_wait) / 1e3)
             tail.append((int(m[live, 3].max()) - int(m[live, 2].max())) / 1e3)
-        rows.append({"reduce": "cluster/dsmem" if cluster == "1" else "global memory", "k_splits_requested": ks, "ctas": ctas, "us_per_launch": round(us, 2), "tbs": round(N * K * 2 / us / 1e6, 2),
+        rows.append({"k_splits_requested": ks, "ctas": ctas, "us_per_launch": round(us, 2), "tbs": round(N * K * 2 / us / 1e6, 2),
                      "stream_us_median": round(statistics.median(stream), 2), "tail_us_median": round(statistics.median(tail), 2)})
         del g
     os.environ.pop("AF3_KSPLIT", None)
-    os.environ.pop("AF3_CLUSTER_REDUCE", None)
     return {"shape": name, "n_feat": N, "K": K, "epilogue": mode, "weight_bytes": N * K * 2, "ideal_us_at_3350_gbs": round(N * K * 2 / 3350e3, 2),   # H100 SXM data-sheet HBM3 bandwidth
             "sweep": rows}
 

@@ -31,7 +31,7 @@ def test_every_declared_symbol_is_exported(lib):
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in af3b200.h but not exported"
     assert sorted(_lib.SIGNATURES) == syms, "ctypes signature table and header disagree"
-    assert lib.af3_abi_version() == 3   # v2: trace API, af3_gemm_bf16_fused, fusion argument of af3_gemm_qkv_rope; v3: af3_gated_residual, af3_token_step
+    assert lib.af3_abi_version() == 4   # v2: trace API; v3: af3_gated_residual, af3_token_step; v4: RMSNorm fusion removed
 
 
 def test_library_contains_hopper_instructions():

@@ -303,32 +303,3 @@ def test_generate_reuses_decode_graph_across_calls(O):
     assert not torch.equal(lw, la1)
     ours.release_decode_state()
     assert ours._decode_state is None
-
-
-def test_fused_rmsnorm_decode_matches_unfused_chain(O, monkeypatch):
-    """AF3_FUSE_NORM=1 (RMSNorm fused across the decode step's GEMMs; opt-in, measured slower) vs 0 (stand-alone norm kernels):
-    same greedy ids; logits within bf16 noise of each other; CUDA-graph replay of the fused chain == its eager execution bit for bit."""
-    from audio_flamingo_b200 import AudioFlamingo3ForConditionalGeneration
-
-    ref32 = O.hf_model("mid", seed=4, sharpen=8.0)
-    cfg = ref32.config
-    waves, feats, fmask, ids, am = _inputs(O, cfg, [30.0, 9.0, 2.0], seed=17)
-    ours = AudioFlamingo3ForConditionalGeneration.from_reference(ref32, device="cuda")
-    kw = dict(input_ids=ids.cuda(), attention_mask=am.cuda(), input_features=feats.cuda(), input_features_mask=fmask.cuda(),
-              max_new_tokens=12, return_logits=True)
-    monkeypatch.setenv("AF3_FUSE_NORM", "1")
-    g1, l1 = ours.generate(**kw)
-    g1e, l1e = ours.generate(use_cuda_graph=False, **kw)
-    assert torch.equal(g1, g1e) and torch.equal(l1, l1e)
-    monkeypatch.setenv("AF3_FUSE_NORM", "0")
-    g0, l0 = ours.generate(**kw)
-    err = (l1 - l0).abs().max().item()
-    print(f"fused vs unfused RMSNorm decode: max |logit diff| {err:.4f}, logit std {l0.std().item():.3f}")
-    assert err <= 0.02 * l0.std().item()
-    S = ids.shape[1]
-    same = (g1[:, S:] == g0[:, S:])
-    for b in range(same.shape[0]):
-        if not bool(same[b].all()):
-            t = int((~same[b]).nonzero()[0])
-            top2 = l0[b, t].topk(2).values
-            assert (top2[0] - top2[1]).item() < 0.05 * l0[b, t].std().item()
