@@ -3,19 +3,28 @@
 // Replaces the cuBLASLt calls behind  F.linear / F.conv1d  in the reference path
 // ([O] AF3M:111-114,141,153-154,204-205,343-344,398-402; Q2M:41-43,46-48,199-202,474-475).
 //
-// Design (one persistent CTA per SM, 9 warps, warp-specialised):
-//   warp 8      TMA producer: cp.async.bulk.tensor 2-D loads of 128B-swizzled [rows x 64] bf16 tiles into a
-//               STAGES-deep smem ring, completion on mbarriers.
-//   warps 0-7   two consumer warpgroups: wgmma.mma_async (m64 x BN x 16, bf16 -> fp32 in registers) straight from the
-//               ring with smem descriptors, one k-block group kept in flight; each warpgroup owns 64 of the tile's 128
-//               rows.  The finished accumulator goes to an fp32 tile in shared memory, from which the epilogue warps
-//               (4 or 8 of them, one row per lane) apply bias / GELU(erf) / residual / SwiGLU with the reference's bf16
-//               rounding points and store with TMA or vectorised global stores.
-// "Row operand" = the matrix whose rows are the wgmma M dimension (128 per tile), "col operand" = the one whose rows
-// are N (BN).  Normal mode: rows = tokens, cols = features.  Swap mode (few tokens, decode):
-// rows = weight features (so every wgmma streams weight rows), cols = tokens, and the epilogue writes the
-// transposed tile.  Tile order is grouped (GROUP_R row tiles share a col tile) so the 50 MB L2 holds the
-// working set of one wave and HBM sees each operand ~once.
+// Two kernels, one persistent CTA per SM each, picked by the token count:
+//
+// gemm_tok_kernel (normal mode, n_tok > 64; rows = tokens, cols = features), 3 warpgroups, ping-pong:
+//   warpgroup 0    TMA producer: cp.async.bulk.tensor 2-D loads of 128B-swizzled [rows x 64] bf16 tiles into a
+//                  STAGES-deep smem ring, in the CTA's tile order, completion on mbarriers.  Gives its registers to
+//                  the consumers (setmaxnreg).
+//   warpgroups 1-2 consumers, alternate tiles of the CTA: each owns a whole 128 x 128 output tile (two wgmma
+//                  m64n128k16 per k16 step, 128 fp32 accumulators per thread, one k-block group in flight) and runs
+//                  the epilogue straight from the accumulator fragments -- bias / GELU(erf) / residual / SwiGLU with the
+//                  reference's bf16 rounding points -> stmatrix into a 128B-swizzled bf16 slab -> TMA store.  While
+//                  one warpgroup runs its epilogue the other runs its main loop, so the tensor cores stay busy.
+//
+// gemm_kernel (few-token / swap mode, decode), 9 warps:
+//   warp 8         TMA producer, as above.
+//   warps 0-7      two consumer warpgroups: wgmma.mma_async (m64 x BN x 16) straight from the ring, each warpgroup
+//                  owns 64 of the tile's 128 rows.  The finished accumulator goes to an fp32 tile in shared memory,
+//                  from which warps 0-3 (one row per lane) run the epilogue and the split-K reduction.
+//   "Row operand" = the matrix whose rows are the wgmma M dimension (128 per tile) = weight features (so every wgmma
+//   streams weight rows), "col operand" = the tokens (BN = 32); the epilogue writes the transposed tile.
+//
+// Tile order is grouped (GROUP_R row tiles share a col tile) so the 50 MB L2 holds the working set of one wave and
+// HBM sees each operand ~once.
 #include "common.h"
 #include "gemm_epi.h"
 #include "ptx.cuh"
@@ -46,7 +55,7 @@ struct GemmArgs {
     bf16* v_cache;
     const int* rope_pos;     // device int: cache slot of this step
     int rope_H, rope_Hkv, rope_Tmax;
-    int tma_epi;    // normal mode: stage the output tile in smem and write it with TMA (coalesced); residual via TMA too
+    int tma_epi;    // normal mode: stage the output tile in smem and write it with TMA (coalesced); plain residual via TMA too
     // SwiGLU weight layout: 0 = gate / up interleaved in blocks of 128 rows (af3_pack_gate_up); > 0 = plain concatenation
     // [gate (n_feat rows); up (n_feat rows)], the value being the first up row -- the two 128-row halves of a tile are then fetched
     // by two TMA boxes, and gate_proj.weight / up_proj.weight can simply be VIEWS of the fused matrix (no second copy in HBM)
@@ -58,9 +67,34 @@ struct GemmArgs {
 };
 
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
-constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma + epilogue), warp 8: TMA producer
 
-template <int BN, int NA, int STAGES, bool SWAP>
+template <int V>
+struct IntC {
+    static constexpr int value = V;
+};
+
+// ---- normal mode
+constexpr int TOK_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: ping-pong consumers
+// Ring depth, chosen by measurement on an H100 80GB HBM3 (700 W): 4 stages ran the prefill GEMMs 3-10 % faster than 5 (the
+// most that fits beside the 64 KB of output slabs) -- e.g. SwiGLU gate/up 24960 x 37888 x 3584 at 618-624 TFLOP/s against
+// 572-574 -- while the encoder's K = 1280 GEMMs moved by 1-4 % either way.
+constexpr int TOK_STAGES = 4;
+
+template <int STAGES>
+struct TokCfg {
+    static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
+    static constexpr int STAGE_BYTES = 2 * X_BYTES;      // + 128 weight rows x 64
+    static constexpr int SLAB_BYTES = 128 * 128;         // [128 rows][64 bf16] 128B-swizzled output / residual slab
+    static constexpr int STAGING_BYTES = 2 * 2 * SLAB_BYTES;  // per consumer warpgroup: the 128 output columns of its tile
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert((2 * STAGES + 4) * 8 <= 256, "barrier area");
+    static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
+};
+
+// ---- few-token (swap) mode
+constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma; warps 0-3 also run the epilogue), warp 8: TMA producer
+
+template <int BN, int NA, int STAGES>
 struct GemmCfg {
     static constexpr int R_BYTES = 128 * NA * BK * 2;
     static constexpr int C_BYTES = BN * BK * 2;
@@ -68,12 +102,11 @@ struct GemmCfg {
     static constexpr int ACC_COLS = NA * BN;
     // the finished fp32 accumulator tile [128 rows][ACC_COLS], handed from the wgmma registers to the epilogue warps
     static constexpr int ACC_BYTES = 128 * ACC_COLS * 4;
-    // normal mode: 4 epilogue warps x 2 buffers x (32 rows x 128 B) staging for the TMA-store epilogue
-    // swap mode: one [32 tokens x 128 features] bf16 tile to transpose the accumulator for token-major vector I/O
-    static constexpr int EPI_STAGE_BYTES = SWAP ? 32 * 128 * 2 : 4 * 2 * 4096;
+    // one [32 tokens x 128 features] bf16 tile to transpose the accumulator for token-major vector I/O
+    static constexpr int EPI_STAGE_BYTES = 32 * 128 * 2;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-    static_assert((2 * STAGES + 8) * 8 + 16 <= 256, "barrier area");
-    static_assert(BN == 32 || BN == 128, "BN: wgmma shapes m64n32 / m64n128");
+    static_assert(2 * STAGES * 8 + 16 <= 256, "barrier area");
+    static_assert(BN == 32, "BN: wgmma shape m64n32");
     static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
 };
 
@@ -121,24 +154,302 @@ __device__ __forceinline__ float epi_swiglu(float g, float u) {
     return bf16_round(s * u);
 }
 
+// ============================================================================ normal mode (n_tok > 64)
+// EPI >= 0: epilogue flags fixed at compile time (no per-element branches); EPI < 0: generic instantiation reading
+// a.flags at run time (odd layouts / unusual flag mixes).
+//
+// Ring protocol.  The producer fills the ring with the k-blocks of the CTA's tiles in order; the tile with local index j
+// (j = 0, 1, ...; global tile blockIdx.x + j * gridDim.x) belongs to consumer warpgroup j % 2, and its k-blocks are ring
+// slots j * kb_n ... (j + 1) * kb_n - 1, so each consumer derives stage and phase of its tile and skips the other's.
+// mbarrier parity waits are only sound for a waiter at most one phase ahead of the barrier, so the consumers start their
+// main loops in tile order: consumer j % 2 begins tile j once the other has issued all of tile j - 1 (barrier `order`).
+// That is the ping-pong: the other warpgroup's epilogue overlaps this one's main loop.
+template <int STAGES, int EPI>
+__global__ void __launch_bounds__(TOK_THREADS, 1)
+gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+                const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
+    using Cfg = TokCfg<STAGES>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+    uint64_t* empty = full + STAGES;
+    uint64_t* order = empty + STAGES;  // [2] one completion per main loop of consumer 0 / 1
+    uint64_t* rbar = order + 2;        // [2] residual slabs of consumer 0 / 1 have landed
+
+    const int wg = threadIdx.x >> 7;
+    const int tw = threadIdx.x & 127;
+    const int flags = (EPI >= 0) ? EPI : a.flags;
+    const bool swiglu = flags & EPI_SWIGLU;
+    const bool tma_res = a.tma_epi && (flags & EPI_RESID) && a.res_period == 0;
+
+    if (threadIdx.x == 0) {
+        trace_mark(a.trace, 0);
+        tma_prefetch_desc(&map_x);
+        tma_prefetch_desc(&map_w);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], 4);  // one arrival per warp of the consuming warpgroup
+        }
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(&order[i], 1);
+            mbar_init(&rbar[i], 1);
+        }
+        if (a.tma_epi) {
+            tma_prefetch_desc(&map_out);
+            if (tma_res) tma_prefetch_desc(&map_res);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();  // the next kernel may start its prologue behind us
+
+    const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+    const int kb_n = (a.K + BK - 1) / BK;
+
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tw == 0) {
+            // SwiGLU tile c (output features [64c, 64c + 64)): the 64 gate rows, then the 64 up rows of the same features --
+            // 128 rows later (gate / up interleaved in blocks of 128 rows) or at swiglu_up_row0 + 64c ([gate; up])
+            auto gate_row = [&](int c) { return a.swiglu_up_row0 ? c * 64 : (c >> 1) * 256 + (c & 1) * 64; };
+            auto up_row = [&](int c) { return a.swiglu_up_row0 ? a.swiglu_up_row0 + c * 64 : gate_row(c) + 128; };
+            pdl_wait();
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+                int r, c;
+                tile_coords(t, a, r, c);
+                for (int kb = 0; kb < kb_n; ++kb) {
+                    uint8_t* sX = smem + stage * Cfg::STAGE_BYTES;
+                    uint8_t* sW = sX + Cfg::X_BYTES;
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+                    tma_load_2d(sX, &map_x, &full[stage], kb * BK, r * 128);
+                    if (swiglu) {
+                        tma_load_2d(sW, &map_w, &full[stage], kb * BK, gate_row(c));
+                        tma_load_2d(sW + 64 * BK * 2, &map_w, &full[stage], kb * BK, up_row(c));
+                    } else {
+                        tma_load_2d(sW, &map_w, &full[stage], kb * BK, c * 128);
+                    }
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+            }
+        }
+    } else {
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;  // consumer index
+        const int warp = tw >> 5, lane = tw & 31;
+        uint8_t* stg = staging + cw * 2 * Cfg::SLAB_BYTES;
+        const uint32_t stg_u32 = smem_u32(stg);
+        const bool leader = tw == 0;
+        const int n_slabs = swiglu ? 1 : 2;  // 64-column output slabs per tile
+        // accumulator fragment acc[h][i]: tile row h * 64 + 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
+        const int frow = warp * 16 + (lane >> 2);
+        const int fcol = 2 * (lane & 3);
+        // stmatrix / ldmatrix x4 over column groups (2 n2, 2 n2 + 1) x rows (+0, +8): this lane addresses row
+        // 16 warp + 8 ((lane >> 3) & 1) + lane % 8 of the 64-row half, column group 2 n2 + (lane >> 4)
+        const int mrow = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+        const int mcg = lane >> 4;
+        auto slab_addr = [&](int row, int cg) {  // 16-byte chunk (row, column group cg of the tile) in the swizzled slabs
+            return stg_u32 + (cg >> 3) * Cfg::SLAB_BYTES + row * 128 + (((cg & 7) ^ (row & 7)) << 4);
+        };
+        const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
+        const bool res_vec = (reinterpret_cast<uintptr_t>(a.resid) & 3) == 0 && (a.ld_res & 1) == 0;
+        // two consecutive bf16 of a row vector (bias / residual row) as floats; zero past n
+        auto ld2 = [&](const bf16* p, int col, bool vec) {
+            if (vec && col + 1 < a.n_feat) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + col));
+            return make_float2(col < a.n_feat ? __bfloat162float(p[col]) : 0.f, col + 1 < a.n_feat ? __bfloat162float(p[col + 1]) : 0.f);
+        };
+        pdl_wait();  // residual reads / output writes are ordered after every earlier kernel
+        if (threadIdx.x == 128) trace_mark(a.trace, 1);
+        uint32_t rpar = 0;
+        for (int j = cw;; j += 2) {
+            const int t = blockIdx.x + j * gridDim.x;
+            if (t >= num_tiles) break;
+            int r, c;
+            tile_coords(t, a, r, c);
+            const int out_col0 = c * (swiglu ? 64 : 128);
+            if (tma_res && leader) {  // residual slabs of this tile: they arrive while the main loop runs
+                bulk_wait_read<0>();  // the previous tile's store has read the staging slabs
+                const int ns = (out_col0 + 64 < a.n_feat) ? 2 : 1;
+                mbar_arrive_expect_tx(&rbar[cw], ns * Cfg::SLAB_BYTES);
+                for (int s = 0; s < ns; ++s) tma_load_2d(stg + s * Cfg::SLAB_BYTES, &map_res, &rbar[cw], out_col0 + 64 * s, r * 128);
+            }
+
+            // ---- main loop: 128 x 128 tile, two m64n128k16 per k16 step (rows 0-63, rows 64-127)
+            float acc[2][64];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+            if (j > 0) mbar_wait(&order[cw ^ 1], ((j - 1) >> 1) & 1);  // tile j - 1 fully issued by the other consumer
+            const int g0 = j * kb_n;  // ring slot of this tile's first k-block
+            int stage = g0 % STAGES;
+            uint32_t phase = (g0 / STAGES) & 1;
+            int prev = -1;
+            for (int kb = 0; kb < kb_n; ++kb) {
+                mbar_wait(&full[stage], phase);
+                const uint32_t sX = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+                const uint32_t sW = sX + Cfg::X_BYTES;
+                fence_regs(acc[0]);
+                fence_regs(acc[1]);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t bdesc = make_smem_desc_sw128(sW + k * 32, 0, 1024);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        wgmma_m64n128_ss<0, 0>(acc[h], make_smem_desc_sw128(sX + h * 64 * 128 + k * 32, 0, 1024), bdesc, 1);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
+                fence_regs(acc[0]);
+                fence_regs(acc[1]);
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == STAGES) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+            if (leader) mbar_arrive(&order[cw]);  // every full-barrier wait of this tile is behind us: the other consumer may start
+            wgmma_wait<0>();
+            fence_regs(acc[0]);
+            fence_regs(acc[1]);
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            if (threadIdx.x == 128) trace_mark(a.trace, 2);
+
+            // ---- epilogue from the accumulator fragments
+            // the compile-time epilogues are launched only with the TMA-store path (launch_normal); the direct-store fallback
+            // exists in the generic instantiation alone, which keeps the specialised kernels small
+            if (EPI >= 0 || a.tma_epi) {
+                if (!tma_res && leader) bulk_wait_read<0>();
+                named_bar_sync(1 + cw, 128);  // the previous tile's store has read the staging slabs
+                if (tma_res) {
+                    mbar_wait(&rbar[cw], rpar);
+                    rpar ^= 1;
+                }
+                // one unrolled pass over the tile per residual source, so that each pass holds only its own operands
+                auto stage_tile = [&](auto res_src) {  // 0: none, 1: slab in smem (TMA), 2: periodic rows from global memory
+                    constexpr int RES = decltype(res_src)::value;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const bf16* rp[2] = {a.resid, a.resid};
+                        if constexpr (RES == 2) {
+                            const int rr0 = (r * 128 + h * 64 + frow) % a.res_period;
+                            rp[0] += static_cast<size_t>(rr0) * a.ld_res;
+                            rp[1] += static_cast<size_t>((rr0 + 8) % a.res_period) * a.ld_res;
+                        }
+#pragma unroll
+                        for (int n2 = 0; n2 < (swiglu ? 4 : 8); ++n2) {
+                            const uint32_t maddr = slab_addr(h * 64 + mrow, 2 * n2 + mcg);
+                            uint32_t rr[4];
+                            if constexpr (RES == 1) ldmatrix_x4(maddr, rr);  // residual pairs in the accumulator's fragment layout
+                            uint32_t y[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) {
+                                const int cg = 2 * n2 + (q >> 1);  // column group; q & 1: rows +0 / +8
+                                const int i = 4 * cg + 2 * (q & 1);
+                                if (swiglu) {
+                                    y[q] = pack_bf16x2(epi_swiglu(acc[h][i], acc[h][i + 32]), epi_swiglu(acc[h][i + 1], acc[h][i + 33]));
+                                } else {
+                                    const int col = out_col0 + 8 * cg + fcol;
+                                    const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, bias_vec) : make_float2(0.f, 0.f);
+                                    float2 res = make_float2(0.f, 0.f);
+                                    if constexpr (RES == 1) res = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rr[q]));
+                                    if constexpr (RES == 2) res = ld2(rp[q & 1], col, res_vec);
+                                    y[q] = pack_bf16x2(epi_elem(acc[h][i], flags, b.x, res.x), epi_elem(acc[h][i + 1], flags, b.y, res.y));
+                                }
+                            }
+                            stmatrix_x4(maddr, y[0], y[1], y[2], y[3]);
+                        }
+                    }
+                };
+                if (tma_res)
+                    stage_tile(IntC<1>{});
+                else if (flags & EPI_RESID)  // periodic residual (positional embedding)
+                    stage_tile(IntC<2>{});
+                else
+                    stage_tile(IntC<0>{});
+                fence_proxy_async_smem();
+                named_bar_sync(1 + cw, 128);
+                if (leader) {
+                    for (int s = 0; s < n_slabs; ++s)
+                        if (out_col0 + 64 * s < a.n_feat) tma_store_2d(&map_out, stg + s * Cfg::SLAB_BYTES, out_col0 + 64 * s, r * 128);
+                    bulk_commit();
+                }
+            } else {
+                // direct stores (output rows not 16-byte aligned, fp32 output): element pairs straight from the fragments
+                const bool out_vec = (reinterpret_cast<uintptr_t>(a.out) & ((flags & EPI_F32OUT) ? 7 : 3)) == 0 && (a.ldo & 1) == 0;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int p = 0; p < 2; ++p) {
+                        const int tok = r * 128 + h * 64 + frow + 8 * p;
+                        if (tok >= a.n_tok) continue;
+                        const int res_row = (a.res_period > 0) ? tok % a.res_period : tok;
+#pragma unroll
+                        for (int cg = 0; cg < (swiglu ? 8 : 16); ++cg) {
+                            const int i = 4 * cg + 2 * p;
+                            const int col = out_col0 + 8 * cg + fcol;
+                            if (col >= a.n_feat) continue;
+                            float2 v;
+                            if (swiglu) {
+                                v = make_float2(epi_swiglu(acc[h][i], acc[h][i + 32]), epi_swiglu(acc[h][i + 1], acc[h][i + 33]));
+                            } else {
+                                const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, bias_vec) : make_float2(0.f, 0.f);
+                                const float2 res = (flags & EPI_RESID) ? ld2(a.resid + static_cast<size_t>(res_row) * a.ld_res, col, res_vec)
+                                                                       : make_float2(0.f, 0.f);
+                                v = make_float2(epi_elem(acc[h][i], flags, b.x, res.x), epi_elem(acc[h][i + 1], flags, b.y, res.y));
+                            }
+                            const size_t o = static_cast<size_t>(tok) * a.ldo + col;
+                            const bool pair = out_vec && col + 1 < a.n_feat;
+                            if (flags & EPI_F32OUT) {
+                                float* op = reinterpret_cast<float*>(a.out) + o;
+                                if (pair) {
+                                    *reinterpret_cast<float2*>(op) = v;
+                                } else {
+                                    op[0] = v.x;
+                                    if (col + 1 < a.n_feat) op[1] = v.y;
+                                }
+                            } else {
+                                bf16* op = reinterpret_cast<bf16*>(a.out) + o;
+                                if (pair) {
+                                    *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v.x, v.y);
+                                } else {
+                                    op[0] = __float2bfloat16_rn(v.x);
+                                    if (col + 1 < a.n_feat) op[1] = __float2bfloat16_rn(v.y);
+                                }
+                            }
+                        }
+                    }
+                }
+            }
+        }
+        if (leader) bulk_wait_read<0>();  // staged tiles must be read out before shared memory goes away
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) trace_mark(a.trace, 3);
+}
+
+// ============================================================================ few-token (swap) mode (n_tok <= 64)
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches, full ILP across the 32-column chunk);
 // EPI < 0: generic instantiation reading a.flags at run time (odd layouts / unusual flag mixes).
-// EW = epilogue warps (4 or 8) among the 8 consumer warps.  With 8 (normal mode, epilogues without a TMA-prefetched residual) two
-// warps share each 32-row quarter of the tile and split its 64-column groups between them: twice the issue slots for epilogue
-// math, which is what bounds short-K GEMMs with expensive epilogues (K = 1280 + GELU: erff per element).
-template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW>
+template <int BN, int NA, int STAGES, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_c,
-            const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
-    using Cfg = GemmCfg<BN, NA, STAGES, SWAP>;
+gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_c, const GemmArgs a) {
+    using Cfg = GemmCfg<BN, NA, STAGES>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     float* accbuf = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint8_t* epi_stage = smem + STAGES * Cfg::STAGE_BYTES + Cfg::ACC_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(epi_stage + Cfg::EPI_STAGE_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* rbar = empty + STAGES;  // [4 warps][2 buffers] residual-tile arrival
-    uint32_t* flag_slot = reinterpret_cast<uint32_t*>(rbar + 8);
+    uint32_t* flag_slot = reinterpret_cast<uint32_t*>(empty + STAGES);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -152,34 +463,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             mbar_init(&full[i], 1);
             mbar_init(&empty[i], 8);  // one arrival per consumer warp
         }
-        for (int i = 0; i < 8; ++i) mbar_init(&rbar[i], 1);
-        if (a.tma_epi) {
-            tma_prefetch_desc(&map_out);
-            if ((flags & EPI_RESID) && a.res_period == 0) tma_prefetch_desc(&map_res);
-        }
         fence_barrier_init();
     }
     __syncthreads();
     pdl_launch_dependents();  // the next kernel may start its prologue / weight prefetch behind us
 
-    const int k_splits = SWAP ? a.k_splits : 1;
+    const int k_splits = a.k_splits;
     const int num_tiles = a.num_r_tiles * a.num_c_tiles * k_splits;  // work items: (tile, split), split fastest
     const int k_blocks_total = (a.K + BK - 1) / BK;
     // K range of split s: blocks [kb_lo(s), kb_lo(s+1)), sizes differ by at most one
     auto kb_lo = [&](int s) { return (s * k_blocks_total) / k_splits; };
-    // row of the col operand where the 64 gate rows (normal-mode SwiGLU tile c: output features [64c, 64c + 64)) start; the 64 up
-    // rows follow 128 rows later (gate / up interleaved in blocks of 128 rows) or at swiglu_up_row0 + 64c ([gate; up])
-    auto gate_row = [&](int c) { return a.swiglu_up_row0 ? c * 64 : (c >> 1) * 256 + (c & 1) * 64; };
-    auto up_row = [&](int c) { return a.swiglu_up_row0 ? a.swiglu_up_row0 + c * 64 : gate_row(c) + 128; };
 
     if (warp == 8) {
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            // Swap mode: the row operand is a WEIGHT matrix, independent of earlier kernels -> its first STAGES tiles are
+            // The row operand is a WEIGHT matrix, independent of earlier kernels -> its first STAGES tiles are
             // requested before pdl_wait(), so weight streaming overlaps the tail of the previous kernel(s).
             int prefetched = 0;
-            if constexpr (SWAP) {
+            {
                 const int t0 = blockIdx.x;
                 if (t0 < num_tiles) {
                     int r, c;
@@ -210,14 +512,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
                             tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[stage], kb * BK,
-                                        (SWAP && a.swiglu_up_row0) ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
+                                        a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
-                    if (!SWAP && (flags & EPI_SWIGLU)) {   // 64 gate rows, then the 64 up rows of the same output features
-                        tma_load_2d(sC, &map_c, &full[stage], kb * BK, gate_row(c));
-                        tma_load_2d(sC + 64 * BK * 2, &map_c, &full[stage], kb * BK, up_row(c));
-                    } else {
-                        tma_load_2d(sC, &map_c, &full[stage], kb * BK, c * BN);
-                    }
+                    tma_load_2d(sC, &map_c, &full[stage], kb * BK, c * BN);
                     if (++stage == STAGES) {
                         stage = 0;
                         phase ^= 1;
@@ -232,15 +529,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
         const int wg = warp >> 2;
         const int tw = threadIdx.x & 127;   // thread within the warpgroup
         const int q = warp & 3;             // 32-row quarter of the tile this warp's epilogue owns
-        [[maybe_unused]] const int ehalf = (EW == 8) ? wg : 0;  // which half of the column groups (EW == 8)
         const int row_in_tile = q * 32 + lane;
-        const bool epi_warp = warp < EW;
+        const bool epi_warp = warp < 4;
         pdl_wait();  // residual reads / output writes / split-K workspace are ordered after every earlier kernel
         if (threadIdx.x == 0) trace_mark(a.trace, 1);
         int stage = 0;
         uint32_t phase = 0;
-        uint32_t egrp = 0;             // running 64-column group counter of this warp (selects the staging buffer)
-        uint32_t rpar0 = 0, rpar1 = 0;  // residual-barrier parities per buffer
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
             {
                 const int sp = t % k_splits;
@@ -264,10 +558,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 #pragma unroll
                         for (int na = 0; na < NA; ++na) {
                             const uint64_t adesc = make_smem_desc_sw128(sR + na * 128 * BK * 2 + wg * 64 * 128 + k * 32, 0, 1024);
-                            if constexpr (BN == 128)
-                                wgmma_m64n128_ss<0, 0>(accr[na], adesc, bdesc, 1);
-                            else
-                                wgmma_m64n32_ss<0, 0>(accr[na], adesc, bdesc, 1);
+                            wgmma_m64n32_ss<0, 0>(accr[na], adesc, bdesc, 1);
                         }
                     }
                     wgmma_commit();
@@ -297,24 +588,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             if (!epi_warp) continue;
             int r, c;
             tile_coords(t / k_splits, a, r, c);
-            [[maybe_unused]] const bool swiglu = flags & EPI_SWIGLU;
-            [[maybe_unused]] const bool tma_res = a.tma_epi && (flags & EPI_RESID) && a.res_period == 0;
-            [[maybe_unused]] const int out_col_base = c * (swiglu ? BN / 2 : BN);
-            [[maybe_unused]] const int row0 = r * 128 + q * 32;
-            if constexpr (!SWAP) {
-                if (tma_res && lane == 0) {  // prefetch the residual slab of group 0 while the accumulator is still in flight
-                    bulk_wait_read<0>();
-                    const int b0 = egrp & 1;
-                    mbar_arrive_expect_tx(&rbar[q * 2 + b0], 4096);
-                    tma_load_2d(epi_stage + (q * 2 + b0) * 4096, &map_res, &rbar[q * 2 + b0], out_col_base, row0);
-                }
-            }
             // few-token mode with a fused residual: this thread's residual vectors of the transposed epilogue (token et / 4,
             // features (et % 4) * 32 ...) do not depend on this GEMM -- request them now, they arrive while the weights stream
             // (the epilogue otherwise exposes one more L2 round trip in the split-K tail)
             [[maybe_unused]] uint4 rv_pre[4];
             [[maybe_unused]] bool rv_ok = false;
-            if constexpr (SWAP && BN == 32 && NA == 1) {
+            if constexpr (BN == 32 && NA == 1) {
                 if ((flags & EPI_RESID) && !(flags & EPI_F32OUT) && (a.ldo & 7) == 0 && (a.ld_res & 7) == 0 && a.res_period == 0) {
                     const int et = threadIdx.x;
                     const int tok = c * BN + (et >> 2);
@@ -329,214 +608,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             }
             if (threadIdx.x == 0) trace_mark(a.trace, 2);
 
-            if constexpr (!SWAP) {
-                const int tok = r * 128 + row_in_tile;
-                const bool row_ok = tok < a.n_tok;
-                const int res_row = (a.res_period > 0) ? (tok % a.res_period) : tok;
-                if (a.tma_epi) {
-                    // ---- smem-staged epilogue: per warp, 64 output columns at a time -> [32 rows x 128 B] swizzled slab -> TMA store
-                    const int n_groups = (swiglu ? BN / 2 : BN) / 64;
-                    // EW == 8: this warp owns half of the groups and ONE staging buffer (index ehalf); EW == 4: all groups,
-                    // two alternating buffers
-                    const int g_lo = (EW == 8) ? ehalf * (n_groups / 2) : 0;
-                    const int g_hi = (EW == 8) ? g_lo + n_groups / 2 : n_groups;
-#pragma unroll 1
-                    for (int gi = g_lo; gi < g_hi; ++gi) {
-                        const int buf = (EW == 8) ? ehalf : (egrp & 1);
-                        uint8_t* sbuf = epi_stage + (q * 2 + buf) * 4096;
-                        if (out_col_base + gi * 64 >= a.n_feat) break;  // fully out-of-range group (warp-uniform)
-                        if (lane == 0) {
-                            if (tma_res) {
-                                bulk_wait_read<0>();  // store of the previous group has drained its buffer
-                                if (gi + 1 < n_groups && out_col_base + (gi + 1) * 64 < a.n_feat) {
-                                    mbar_arrive_expect_tx(&rbar[q * 2 + (buf ^ 1)], 4096);
-                                    tma_load_2d(epi_stage + (q * 2 + (buf ^ 1)) * 4096, &map_res, &rbar[q * 2 + (buf ^ 1)],
-                                                out_col_base + (gi + 1) * 64, row0);
-                                }
-                            } else if (EW == 8) {
-                                bulk_wait_read<0>();  // single buffer per warp: the previous store has drained it
-                            } else {
-                                bulk_wait_read<1>();  // the store that last used THIS buffer has drained it
-                            }
-                        }
-                        __syncwarp();
-                        if (tma_res) {
-                            mbar_wait(&rbar[q * 2 + buf], buf ? rpar1 : rpar0);
-                            if (buf) rpar1 ^= 1; else rpar0 ^= 1;
-                        }
-                        uint8_t* srow = sbuf + lane * 128;
-#pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            const int tcol = gi * 64 + half * 32;
-                            uint32_t v[32], u[32];
-                            acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, tcol, v);
-                            if (swiglu) acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, BN / 2 + tcol, u);
-                            const int f0 = out_col_base + tcol;
-                            float x[32];
-                            if (swiglu) {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) x[j] = epi_swiglu(__uint_as_float(v[j]), __uint_as_float(u[j]));
-                            } else {
-                                float bsv[32], rs[32];
-                                if ((flags & EPI_BIAS) && f0 + 32 <= a.n_feat) {
-                                    const uint4* bp = reinterpret_cast<const uint4*>(a.bias + f0);
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        uint4 bv = __ldg(bp + j);
-                                        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&bv);
-#pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            float2 f = __bfloat1622float2(h[e]);
-                                            bsv[j * 8 + e * 2] = f.x;
-                                            bsv[j * 8 + e * 2 + 1] = f.y;
-                                        }
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j)
-                                        bsv[j] = ((flags & EPI_BIAS) && f0 + j < a.n_feat) ? __bfloat162float(a.bias[f0 + j]) : 0.f;
-                                }
-                                if (tma_res) {
-#pragma unroll
-                                    for (int g4 = 0; g4 < 4; ++g4) {
-                                        const uint4 rv = *reinterpret_cast<const uint4*>(srow + (((half * 4 + g4) ^ (lane & 7)) << 4));
-                                        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            float2 f = __bfloat1622float2(h[e]);
-                                            rs[g4 * 8 + e * 2] = f.x;
-                                            rs[g4 * 8 + e * 2 + 1] = f.y;
-                                        }
-                                    }
-                                } else if (flags & EPI_RESID) {  // periodic residual (positional embedding): direct loads
-                                    const bf16* rp = a.resid + static_cast<size_t>(res_row) * a.ld_res + f0;
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) rs[j] = (row_ok && f0 + j < a.n_feat) ? __bfloat162float(rp[j]) : 0.f;
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) rs[j] = 0.f;
-                                }
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) x[j] = epi_elem(__uint_as_float(v[j]), flags, bsv[j], rs[j]);
-                            }
-#pragma unroll
-                            for (int g4 = 0; g4 < 4; ++g4)
-                                *reinterpret_cast<uint4*>(srow + (((half * 4 + g4) ^ (lane & 7)) << 4)) =
-                                    make_uint4(pack_bf16x2(x[8 * g4], x[8 * g4 + 1]), pack_bf16x2(x[8 * g4 + 2], x[8 * g4 + 3]),
-                                               pack_bf16x2(x[8 * g4 + 4], x[8 * g4 + 5]), pack_bf16x2(x[8 * g4 + 6], x[8 * g4 + 7]));
-                        }
-                        fence_proxy_async_smem();
-                        __syncwarp();
-                        if (lane == 0) {
-                            tma_store_2d(&map_out, sbuf, out_col_base + gi * 64, row0);
-                            bulk_commit();
-                        }
-                        ++egrp;
-                    }
-                } else if (flags & EPI_SWIGLU) {
-                    // cols [0, BN/2) = gate, [BN/2, BN) = up of the same BN/2 output features
-                    constexpr int HALF = BN / 2;
-#pragma unroll 1
-                    for (int ch = 0; ch < HALF / 32; ++ch) {
-                        uint32_t g[32], u[32];
-                        acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, ch * 32, g);
-                        acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, HALF + ch * 32, u);
-                        const int f0 = c * HALF + ch * 32;
-                        if (row_ok && f0 < a.n_feat) {
-                            bf16* o = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                            if (f0 + 32 <= a.n_feat && (a.ldo & 7) == 0) {
-                                uint32_t w[16];
-#pragma unroll
-                                for (int j = 0; j < 16; ++j)
-                                    w[j] = pack_bf16x2(epi_swiglu(__uint_as_float(g[2 * j]), __uint_as_float(u[2 * j])),
-                                                       epi_swiglu(__uint_as_float(g[2 * j + 1]), __uint_as_float(u[2 * j + 1])));
-#pragma unroll
-                                for (int j = 0; j < 4; ++j)
-                                    reinterpret_cast<uint4*>(o)[j] = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-                            } else {
-                                _Pragma("unroll") for (int j = 0; j < 32; ++j) if (f0 + j < a.n_feat)
-                                    o[j] = __float2bfloat16_rn(epi_swiglu(__uint_as_float(g[j]), __uint_as_float(u[j])));
-                            }
-                        }
-                    }
-                } else {
-#pragma unroll 1
-                    for (int ch = 0; ch < BN / 32; ++ch) {
-                        uint32_t v[32];
-                        acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, ch * 32, v);
-                        const int f0 = c * BN + ch * 32;
-                        if (row_ok && f0 < a.n_feat) {
-                            const bool fullv = (f0 + 32 <= a.n_feat);
-                            float x[32];
-                            if (fullv && (flags & EPI_BIAS)) {
-                                const uint4* bp = reinterpret_cast<const uint4*>(a.bias + f0);
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    uint4 bv = __ldg(bp + j);
-                                    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&bv);
-#pragma unroll
-                                    for (int e = 0; e < 4; ++e) {
-                                        float2 f = __bfloat1622float2(h[e]);
-                                        x[j * 8 + e * 2] = f.x;
-                                        x[j * 8 + e * 2 + 1] = f.y;
-                                    }
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j)
-                                    x[j] = ((flags & EPI_BIAS) && f0 + j < a.n_feat) ? __bfloat162float(a.bias[f0 + j]) : 0.f;
-                            }
-                            float rs[32];
-                            if (flags & EPI_RESID) {
-                                const bf16* rp = a.resid + static_cast<size_t>(res_row) * a.ld_res + f0;
-                                if (fullv && (a.ld_res & 7) == 0) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        uint4 rv = *(reinterpret_cast<const uint4*>(rp) + j);
-                                        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            float2 f = __bfloat1622float2(h[e]);
-                                            rs[j * 8 + e * 2] = f.x;
-                                            rs[j * 8 + e * 2 + 1] = f.y;
-                                        }
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) rs[j] = (f0 + j < a.n_feat) ? __bfloat162float(rp[j]) : 0.f;
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) rs[j] = 0.f;
-                            }
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) x[j] = epi_elem(__uint_as_float(v[j]), flags, x[j], rs[j]);
-
-                            if (flags & EPI_F32OUT) {
-                                float* o = reinterpret_cast<float*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                                if (fullv && (a.ldo & 3) == 0) {
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j)
-                                        reinterpret_cast<float4*>(o)[j] = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-                                } else {
-                                    _Pragma("unroll") for (int j = 0; j < 32; ++j) if (f0 + j < a.n_feat) o[j] = x[j];
-                                }
-                            } else {
-                                bf16* o = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                                if (fullv && (a.ldo & 7) == 0) {
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j)
-                                        reinterpret_cast<uint4*>(o)[j] =
-                                            make_uint4(pack_bf16x2(x[8 * j], x[8 * j + 1]), pack_bf16x2(x[8 * j + 2], x[8 * j + 3]),
-                                                       pack_bf16x2(x[8 * j + 4], x[8 * j + 5]), pack_bf16x2(x[8 * j + 6], x[8 * j + 7]));
-                                } else {
-                                    _Pragma("unroll") for (int j = 0; j < 32; ++j) if (f0 + j < a.n_feat) o[j] = __float2bfloat16_rn(x[j]);
-                                }
-                            }
-                        }
-                    }
-                }
-            } else {
+            {
                 // swapped: accumulator row = output feature, column = token
                 const int feat = r * 128 + row_in_tile;
                 const bool feat_ok = feat < a.n_feat;
@@ -726,53 +798,46 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
         }
     }
 
-    if (!SWAP && warp < EW && lane == 0) bulk_wait_read<0>();  // staged tiles must be read out before smem goes away
     __syncthreads();
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
-template <int BN, int NA, int STAGES, bool SWAP, int EPI, int EW = 4>
-static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMap& mo, const CUtensorMap& mres,
-                  const GemmArgs& a, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, NA, STAGES, SWAP>;
-    auto kern = gemm_kernel<BN, NA, STAGES, SWAP, EPI, EW>;
+template <int EPI>
+static int launch_tok(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
+                      const GemmArgs& a, cudaStream_t stream) {
+    using Cfg = TokCfg<TOK_STAGES>;
+    auto kern = gemm_tok_kernel<TOK_STAGES, EPI>;
     static DeviceOnce once;
     if (once.first()) {
         AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     }
-    const int tiles = a.num_r_tiles * a.num_c_tiles * (SWAP && a.k_splits > 1 ? a.k_splits : 1);
+    const int tiles = a.num_r_tiles * a.num_c_tiles;
     const int grid = tiles < sm_count() ? tiles : sm_count();
-    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, mr, mc, mo, mres, a));
+    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(TOK_THREADS), Cfg::SMEM_BYTES, stream, mx, mw, mo, mres, a));
     return 0;
 }
 
-// Host entry.  x: [n_tok, K] bf16 (pitch ldx), w: [n_rows_w, K] bf16 (pitch ldw) where n_rows_w = n_feat, or the
-// gate/up-interleaved 2*ceil(n_feat/128)*128 rows when EPI_SWIGLU.  out: [n_tok, n_feat] (pitch ldo).
+template <int BN, int NA, int STAGES, int EPI>
+static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const GemmArgs& a, cudaStream_t stream) {
+    using Cfg = GemmCfg<BN, NA, STAGES>;
+    auto kern = gemm_kernel<BN, NA, STAGES, EPI>;
+    static DeviceOnce once;
+    if (once.first()) {
+        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    }
+    const int tiles = a.num_r_tiles * a.num_c_tiles * (a.k_splits > 1 ? a.k_splits : 1);
+    const int grid = tiles < sm_count() ? tiles : sm_count();
+    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, mr, mc, a));
+    return 0;
+}
+
 // compile-time epilogue specialisations for the flag sets the AF3 path uses; anything else -> generic (-1)
-template <int BN, int NA, int STAGES, bool SWAP>
-static int launch(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMap& mo, const CUtensorMap& mres,
-                  const GemmArgs& a, cudaStream_t stream) {
+static int launch_normal(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
+                         const GemmArgs& a, cudaStream_t stream) {
 #define AF3_EPI_CASE(F) \
     case (F):           \
-        return launch_epi<BN, NA, STAGES, SWAP, (F)>(mr, mc, mo, mres, a, stream);
-    if constexpr (!SWAP) {
-        // 8 epilogue warps where the epilogue (not the MMA) bounds the tile: TMA-store path without a TMA residual
-        if (a.tma_epi && !((a.flags & EPI_RESID) && a.res_period == 0)) {
-            switch (a.flags) {
-                case 0:
-                    return launch_epi<BN, NA, STAGES, SWAP, 0, 8>(mr, mc, mo, mres, a, stream);
-                case EPI_BIAS:
-                    return launch_epi<BN, NA, STAGES, SWAP, EPI_BIAS, 8>(mr, mc, mo, mres, a, stream);
-                case EPI_BIAS | EPI_GELU:
-                    return launch_epi<BN, NA, STAGES, SWAP, EPI_BIAS | EPI_GELU, 8>(mr, mc, mo, mres, a, stream);
-                case EPI_BIAS | EPI_GELU | EPI_RESID:
-                    return launch_epi<BN, NA, STAGES, SWAP, EPI_BIAS | EPI_GELU | EPI_RESID, 8>(mr, mc, mo, mres, a, stream);
-                default:
-                    break;
-            }
-        }
-    }
-    if (SWAP || a.tma_epi) {
+        return launch_tok<(F)>(mx, mw, mo, mres, a, stream);
+    if (a.tma_epi) {
         switch (a.flags) {
             AF3_EPI_CASE(0)
             AF3_EPI_CASE(EPI_BIAS)
@@ -780,19 +845,41 @@ static int launch(const CUtensorMap& mr, const CUtensorMap& mc, const CUtensorMa
             AF3_EPI_CASE(EPI_BIAS | EPI_RESID)
             AF3_EPI_CASE(EPI_RESID)
             AF3_EPI_CASE(EPI_SWIGLU)
-            AF3_EPI_CASE(EPI_F32OUT)
             AF3_EPI_CASE(EPI_BIAS | EPI_GELU | EPI_RESID)
-            AF3_EPI_CASE(EPI_BIAS | EPI_ROPE)
             default:
                 break;
         }
     }
 #undef AF3_EPI_CASE
-    return launch_epi<BN, NA, STAGES, SWAP, -1>(mr, mc, mo, mres, a, stream);
+    return launch_tok<-1>(mx, mw, mo, mres, a, stream);
+}
+
+template <int BN, int NA, int STAGES>
+static int launch_swap(const CUtensorMap& mr, const CUtensorMap& mc, const GemmArgs& a, cudaStream_t stream) {
+#define AF3_EPI_CASE(F) \
+    case (F):           \
+        return launch_epi<BN, NA, STAGES, (F)>(mr, mc, a, stream);
+    switch (a.flags) {
+        AF3_EPI_CASE(0)
+        AF3_EPI_CASE(EPI_BIAS)
+        AF3_EPI_CASE(EPI_BIAS | EPI_GELU)
+        AF3_EPI_CASE(EPI_BIAS | EPI_RESID)
+        AF3_EPI_CASE(EPI_RESID)
+        AF3_EPI_CASE(EPI_SWIGLU)
+        AF3_EPI_CASE(EPI_F32OUT)
+        AF3_EPI_CASE(EPI_BIAS | EPI_GELU | EPI_RESID)
+        AF3_EPI_CASE(EPI_BIAS | EPI_ROPE)
+        default:
+            break;
+    }
+#undef AF3_EPI_CASE
+    return launch_epi<BN, NA, STAGES, -1>(mr, mc, a, stream);
 }
 
 size_t gemm_workspace_bytes() { return (8u << 20) + 4096 * sizeof(int); }
 
+// Host entry.  x: [n_tok, K] bf16 (pitch ldx), w: [n_rows_w, K] bf16 (pitch ldw) where n_rows_w = n_feat, or the
+// gate/up-interleaved 2*ceil(n_feat/128)*128 rows when EPI_SWIGLU.  out: [n_tok, n_feat] (pitch ldo).
 int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, void* out, int ldo, int n_tok,
               int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, int res_period,
               void* workspace, size_t workspace_bytes, const RopeEpilogue* rope) {
@@ -855,11 +942,12 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
         mo = mx;
         mres = mx;
         if (a.tma_epi) {
-            if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 32)) return e;
+            // [128 rows x 64 columns] slabs: one TMA store (residual: load) per 64 output columns of a tile
+            if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 128)) return e;
             if (res_plain)
-                if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 32)) return e;
+                if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 128)) return e;
         }
-        return launch<BN, 1, 4, false>(mx, mw, mo, mres, a, stream);
+        return launch_normal(mx, mw, mo, mres, a, stream);
     }
     constexpr int BN = 32;
     a.R = w_rows;
@@ -872,7 +960,7 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
     // allows next to the accumulator tile: the weight streams of a few-token GEMM are latency-bound on the bytes in flight per SM.
     if (swiglu) {
         a.num_r_tiles = ceil_div(w_rows, 256);
-        return launch<BN, 2, 5, true>(mw, mx, mw, mw, a, stream);
+        return launch_swap<BN, 2, 5>(mw, mx, a, stream);
     }
     a.num_r_tiles = ceil_div(w_rows, 128);
     // split-K when the tile grid cannot fill the GPU and a (zero-initialised) workspace was supplied
@@ -892,7 +980,7 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
         }
     }
     // ring depth: 10 x 20 KB = 200 KB in flight per SM (the few-token streams are latency-bound on bytes in flight)
-    return launch<BN, 1, 10, true>(mw, mx, mw, mw, a, stream);
+    return launch_swap<BN, 1, 10>(mw, mx, a, stream);
 }
 
 }  // namespace af3
