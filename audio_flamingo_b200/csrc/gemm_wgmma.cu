@@ -3,9 +3,14 @@
 // Replaces the cuBLASLt calls behind  F.linear / F.conv1d  in the reference path
 // ([O] AF3M:111-114,141,153-154,204-205,343-344,398-402; Q2M:41-43,46-48,199-202,474-475).
 //
-// Two kernels, one persistent CTA per SM each, picked by the token count:
+// Three kernels, one persistent CTA per SM each, picked by the token count and, in normal mode, by K and the epilogue:
 //
-// gemm_tok_kernel (normal mode, n_tok > 64; rows = tokens, cols = features), 3 warpgroups, ping-pong:
+// gemm_tok_wide_kernel (normal mode, K >= 2048, no periodic residual), 3 warpgroups: the producer below, and two consumer
+//                  warpgroups that share each 128 x 256 tile (64 token rows each, one m64n256k16 per k16 step, 3 x 48 KB
+//                  stages).  Sharing the weight slice cuts the shared-memory operand reads and TMA writes per FLOP that
+//                  cap the 128 x 128 tiles; its epilogue is not overlapped, which costs more than it gains at small K.
+//
+// gemm_tok_kernel (normal mode, n_tok > 64, every other case; rows = tokens, cols = features), 3 warpgroups, ping-pong:
 //   warpgroup 0    TMA producer: cp.async.bulk.tensor 2-D loads of 128B-swizzled [rows x 64] bf16 tiles into a
 //                  STAGES-deep smem ring, in the CTA's tile order, completion on mbarriers.  Gives its registers to
 //                  the consumers (setmaxnreg).
@@ -436,6 +441,209 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
+// ============================================================================ normal mode, wide tiles
+// One 128 (tokens) x 256 (weight rows) tile per CTA at a time.  Consumer warpgroup cw owns token rows [64 cw, 64 cw + 64)
+// and all 256 columns: one m64n256k16 per k16 step, 128 fp32 accumulators per thread, and both consumers read the same
+// weight slice, so a k-block moves 48 KB through the ring where two 128 x 128 tiles move 64 KB.  SwiGLU: the 256 weight
+// rows are 128 gate rows then the 128 up rows of the same features, a tile writes 128 output features, and each thread
+// holds gate (acc[i]) and up (acc[i + 64]) of its outputs.  The two consumers finish a tile together, so the epilogue is
+// not hidden behind a main loop; the producer runs ahead into the next tile meanwhile.  Staging: the whole 64 x 256
+// quarter of each consumer (4 slabs of [64 rows x 64 columns]); a plain residual is TMA-loaded into it during the main loop.
+template <int STAGES>
+struct WideCfg {
+    static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
+    static constexpr int W_BYTES = 256 * BK * 2;         // 256 weight rows x 64
+    static constexpr int STAGE_BYTES = X_BYTES + W_BYTES;
+    static constexpr int SLAB_BYTES = 64 * 128;          // [64 rows][64 bf16] 128B-swizzled output / residual slab
+    static constexpr int STAGING_BYTES = 2 * 4 * SLAB_BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert((2 * STAGES + 2) * 8 <= 256, "barrier area");
+    static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
+};
+// 3 x 48 KB stages + 64 KB of staging (≈ 209 KB), chosen by measurement on an H100 80GB HBM3 (700 W): 4 stages with half
+// the staging (two epilogue passes) was as fast within run-to-run spread (prefill GEMMs -1.5 to +5 %, their time-weighted
+// sum 0.5 % slower) and needs the second pass.
+constexpr int WIDE_STAGES = 3;
+
+template <int STAGES, int EPI>
+__global__ void __launch_bounds__(TOK_THREADS, 1)
+gemm_tok_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+                     const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
+    static_assert(EPI >= 0 && !(EPI & EPI_F32OUT), "compile-time epilogue with a TMA store");
+    using Cfg = WideCfg<STAGES>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+    uint64_t* empty = full + STAGES;
+    uint64_t* rbar = empty + STAGES;  // [2] residual slabs of consumer 0 / 1 have landed
+
+    const int wg = threadIdx.x >> 7;
+    const int tw = threadIdx.x & 127;
+    constexpr int flags = EPI;
+    constexpr bool swiglu = flags & EPI_SWIGLU;
+    constexpr int OUT_COLS = swiglu ? 128 : 256;  // output columns of a tile
+    constexpr bool tma_res = flags & EPI_RESID;  // plain residual only (the host keeps periodic ones on the 128 x 128 kernel)
+
+    if (threadIdx.x == 0) {
+        trace_mark(a.trace, 0);
+        tma_prefetch_desc(&map_x);
+        tma_prefetch_desc(&map_w);
+        tma_prefetch_desc(&map_out);
+        if (tma_res) tma_prefetch_desc(&map_res);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], 8);  // one arrival per consumer warp: both warpgroups read every stage
+        }
+        for (int i = 0; i < 2; ++i) mbar_init(&rbar[i], 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();  // the next kernel may start its prologue behind us
+
+    const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+    const int kb_n = (a.K + BK - 1) / BK;
+
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tw == 0) {
+            // weight rows of 128-row half q of column tile c
+            auto w_row = [&](int c, int q) {
+                if (swiglu && a.swiglu_up_row0) return q ? a.swiglu_up_row0 + c * 128 : c * 128;  // [gate; up]
+                return c * 256 + q * 128;  // plain, or one 256-row block of the gate / up interleaved layout
+            };
+            pdl_wait();
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+                int r, c;
+                tile_coords(t, a, r, c);
+                for (int kb = 0; kb < kb_n; ++kb) {
+                    uint8_t* sX = smem + stage * Cfg::STAGE_BYTES;
+                    uint8_t* sW = sX + Cfg::X_BYTES;
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+                    tma_load_2d(sX, &map_x, &full[stage], kb * BK, r * 128);
+                    tma_load_2d(sW, &map_w, &full[stage], kb * BK, w_row(c, 0));
+                    tma_load_2d(sW + Cfg::W_BYTES / 2, &map_w, &full[stage], kb * BK, w_row(c, 1));
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+            }
+        }
+    } else {
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;  // consumer index: token rows [64 cw, 64 cw + 64) of the tile
+        const int warp = tw >> 5, lane = tw & 31;
+        uint8_t* stg = staging + cw * 4 * Cfg::SLAB_BYTES;
+        const uint32_t stg_u32 = smem_u32(stg);
+        const bool leader = tw == 0;
+        // accumulator fragment acc[i]: row 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
+        const int fcol = 2 * (lane & 3);
+        // stmatrix / ldmatrix x4 over column groups (2 n2, 2 n2 + 1) x rows (+0, +8): this lane addresses row
+        // 16 warp + 8 ((lane >> 3) & 1) + lane % 8, column group 2 n2 + (lane >> 4)
+        const int mrow = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+        const int mcg = lane >> 4;
+        auto slab_addr = [&](int row, int cg) {  // 16-byte chunk (row, column group cg) in the swizzled slabs
+            return stg_u32 + (cg >> 3) * Cfg::SLAB_BYTES + row * 128 + (((cg & 7) ^ (row & 7)) << 4);
+        };
+        const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
+        auto ld2 = [&](const bf16* p, int col) {  // two consecutive bias values as floats; zero past n_feat
+            if (bias_vec && col + 1 < a.n_feat) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + col));
+            return make_float2(col < a.n_feat ? __bfloat162float(p[col]) : 0.f, col + 1 < a.n_feat ? __bfloat162float(p[col + 1]) : 0.f);
+        };
+        pdl_wait();  // residual reads / output writes are ordered after every earlier kernel
+        if (threadIdx.x == 128) trace_mark(a.trace, 1);
+        uint32_t rpar = 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+            int r, c;
+            tile_coords(t, a, r, c);
+            const int row0 = r * 128 + cw * 64;  // first token row of this warpgroup
+            const int out_col0 = c * OUT_COLS;
+            if (tma_res && leader) {  // residual slabs of this tile: they arrive while the main loop runs
+                bulk_wait_read<0>();  // the previous tile's store has read the staging slabs
+                int ns = 0;
+                while (ns < 4 && out_col0 + 64 * ns < a.n_feat) ++ns;
+                mbar_arrive_expect_tx(&rbar[cw], ns * Cfg::SLAB_BYTES);
+                for (int s = 0; s < ns; ++s) tma_load_2d(stg + s * Cfg::SLAB_BYTES, &map_res, &rbar[cw], out_col0 + 64 * s, row0);
+            }
+
+            // ---- main loop: one m64n256k16 per k16 step
+            float acc[128];
+#pragma unroll
+            for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+            int prev = -1;
+            for (int kb = 0; kb < kb_n; ++kb) {
+                mbar_wait(&full[stage], phase);
+                const uint32_t sX = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 64 * 128;
+                const uint32_t sW = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::X_BYTES;
+                fence_regs(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)
+                    wgmma_m64n256_ss<0, 0>(acc, make_smem_desc_sw128(sX + k * 32, 0, 1024), make_smem_desc_sw128(sW + k * 32, 0, 1024), 1);
+                wgmma_commit();
+                wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
+                fence_regs(acc);
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = stage;
+                if (++stage == STAGES) {
+                    stage = 0;
+                    phase ^= 1;
+                }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            if (threadIdx.x == 128) trace_mark(a.trace, 2);
+
+            // ---- epilogue from the accumulator fragments
+            if (!tma_res && leader) bulk_wait_read<0>();
+            named_bar_sync(1 + cw, 128);  // the previous tile's store has read the staging slabs
+            if (tma_res) {
+                mbar_wait(&rbar[cw], rpar);
+                rpar ^= 1;
+            }
+#pragma unroll
+            for (int n2 = 0; n2 < OUT_COLS / 16; ++n2) {
+                const uint32_t maddr = slab_addr(mrow, 2 * n2 + mcg);
+                uint32_t rr[4];
+                if constexpr (tma_res) ldmatrix_x4(maddr, rr);  // residual pairs in the accumulator's fragment layout
+                uint32_t y[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int cg = 2 * n2 + (q >> 1);  // column group; q & 1: rows +0 / +8
+                    const int i = 4 * cg + 2 * (q & 1);
+                    if constexpr (swiglu) {
+                        y[q] = pack_bf16x2(epi_swiglu(acc[i], acc[i + 64]), epi_swiglu(acc[i + 1], acc[i + 65]));
+                    } else {
+                        const int col = out_col0 + 8 * cg + fcol;
+                        const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col) : make_float2(0.f, 0.f);
+                        float2 res = make_float2(0.f, 0.f);
+                        if constexpr (tma_res) res = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rr[q]));
+                        y[q] = pack_bf16x2(epi_elem(acc[i], flags, b.x, res.x), epi_elem(acc[i + 1], flags, b.y, res.y));
+                    }
+                }
+                stmatrix_x4(maddr, y[0], y[1], y[2], y[3]);
+            }
+            fence_proxy_async_smem();
+            named_bar_sync(1 + cw, 128);
+            if (leader) {
+                for (int s = 0; s < OUT_COLS / 64; ++s)
+                    if (out_col0 + 64 * s < a.n_feat) tma_store_2d(&map_out, stg + s * Cfg::SLAB_BYTES, out_col0 + 64 * s, row0);
+                bulk_commit();
+            }
+        }
+        if (leader) bulk_wait_read<0>();  // staged tiles must be read out before shared memory goes away
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) trace_mark(a.trace, 3);
+}
+
 // ============================================================================ few-token (swap) mode (n_tok <= 64)
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches, full ILP across the 32-column chunk);
 // EPI < 0: generic instantiation reading a.flags at run time (odd layouts / unusual flag mixes).
@@ -831,21 +1039,43 @@ static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const GemmAr
     return 0;
 }
 
-// compile-time epilogue specialisations for the flag sets the AF3 path uses; anything else -> generic (-1)
+template <int EPI>
+static int launch_wide(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
+                       const GemmArgs& a, cudaStream_t stream) {
+    using Cfg = WideCfg<WIDE_STAGES>;
+    auto kern = gemm_tok_wide_kernel<WIDE_STAGES, EPI>;
+    static DeviceOnce once;
+    if (once.first()) {
+        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    }
+    const int tiles = a.num_r_tiles * a.num_c_tiles;
+    const int grid = tiles < sm_count() ? tiles : sm_count();
+    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(TOK_THREADS), Cfg::SMEM_BYTES, stream, mx, mw, mo, mres, a));
+    return 0;
+}
+
+// compile-time epilogue specialisations for the flag sets the AF3 path uses; anything else -> generic (-1, 128 x 128 tiles)
+#define AF3_TOK_EPIS(X) X(0) X(EPI_BIAS) X(EPI_BIAS | EPI_GELU) X(EPI_BIAS | EPI_RESID) X(EPI_RESID) X(EPI_SWIGLU) \
+    X(EPI_BIAS | EPI_GELU | EPI_RESID)
+static bool tok_epi_specialised(int flags) {
+#define AF3_EPI_CASE(F) case (F):
+    switch (flags) {
+        AF3_TOK_EPIS(AF3_EPI_CASE)
+        return true;
+        default:
+            return false;
+    }
+#undef AF3_EPI_CASE
+}
+
 static int launch_normal(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
-                         const GemmArgs& a, cudaStream_t stream) {
+                         const GemmArgs& a, bool wide, cudaStream_t stream) {
 #define AF3_EPI_CASE(F) \
     case (F):           \
-        return launch_tok<(F)>(mx, mw, mo, mres, a, stream);
+        return wide ? launch_wide<(F)>(mx, mw, mo, mres, a, stream) : launch_tok<(F)>(mx, mw, mo, mres, a, stream);
     if (a.tma_epi) {
         switch (a.flags) {
-            AF3_EPI_CASE(0)
-            AF3_EPI_CASE(EPI_BIAS)
-            AF3_EPI_CASE(EPI_BIAS | EPI_GELU)
-            AF3_EPI_CASE(EPI_BIAS | EPI_RESID)
-            AF3_EPI_CASE(EPI_RESID)
-            AF3_EPI_CASE(EPI_SWIGLU)
-            AF3_EPI_CASE(EPI_BIAS | EPI_GELU | EPI_RESID)
+            AF3_TOK_EPIS(AF3_EPI_CASE)
             default:
                 break;
         }
@@ -853,6 +1083,7 @@ static int launch_normal(const CUtensorMap& mx, const CUtensorMap& mw, const CUt
 #undef AF3_EPI_CASE
     return launch_tok<-1>(mx, mw, mo, mres, a, stream);
 }
+#undef AF3_TOK_EPIS
 
 template <int BN, int NA, int STAGES>
 static int launch_swap(const CUtensorMap& mr, const CUtensorMap& mc, const GemmArgs& a, cudaStream_t stream) {
@@ -947,7 +1178,19 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
             if (res_plain)
                 if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 128)) return e;
         }
-        return launch_normal(mx, mw, mo, mres, a, stream);
+        // 128 x 256 tiles where the main loop is long enough to pay for an epilogue that no main loop hides.  On an H100
+        // 80GB HBM3 (700 W) they ran every K >= 3584 GEMM of config 2 7-15 % faster than the ping-pong kernel, but conv2
+        // (K = 3840, periodic residual read from global memory in the epilogue) 8 % slower, and lost up to 10 % at K = 1280
+        // (profiles/microbench_prefill_gemm.py)
+        const bool wide = a.tma_epi && tok_epi_specialised(flags) && K >= 2048 && res_period == 0;
+        if (wide) {
+            a.num_c_tiles = ceil_div(w_rows, 256);
+            if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, 128)) return e;
+            if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 64)) return e;
+            if (res_plain)
+                if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 64)) return e;
+        }
+        return launch_normal(mx, mw, mo, mres, a, wide, stream);
     }
     constexpr int BN = 32;
     a.R = w_rows;
