@@ -28,6 +28,12 @@
 //   "Row operand" = the matrix whose rows are the wgmma M dimension (128 per tile) = weight features (so every wgmma
 //   streams weight rows), "col operand" = the tokens (BN = 32); the epilogue writes the transposed tile.
 //
+// Shared pieces, written once: the ring cursor (Ring), the consumer k-loop of all three kernels (ring_mma / ring_drain),
+// and for the two token-major kernels the shared-memory carve-up and prologue (TokSmem, tok_prologue), the producer loop
+// (tok_produce; each kernel says how the weight rows of a tile are loaded) and the register epilogue (epi_fragment into
+// OutSlabs, which also load the residual and store the tile by TMA).  All are __forceinline__: a call inside a wgmma
+// kernel makes ptxas serialise every wgmma (C7510).
+//
 // Tile order is grouped (GROUP_R row tiles share a col tile) so the 50 MB L2 holds the working set of one wave and
 // HBM sees each operand ~once.
 #include "common.h"
@@ -39,7 +45,7 @@
 namespace af3 {
 
 struct GemmArgs {
-    int R, C, K;  // extents of row operand, col operand, reduction
+    int K;  // reduction extent
     int num_r_tiles, num_c_tiles, group_r;
     int n_tok, n_feat;  // logical output extents (features after SwiGLU halving)
     void* out;
@@ -78,23 +84,126 @@ struct IntC {
     static constexpr int value = V;
 };
 
+// Position in a STAGES-deep smem ring: the stage, and the parity of the mbarrier phase its current use completes.
+// Ring slot g (the g-th k-block through the ring) is stage g % STAGES in phase (g / STAGES) & 1.
+template <int STAGES>
+struct Ring {
+    int stage;
+    uint32_t phase;
+    __device__ __forceinline__ explicit Ring(int g = 0) : stage(g % STAGES), phase((g / STAGES) & 1) {}
+    __device__ __forceinline__ void next() {
+        if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
+};
+
+// Consumer k-loop of every kernel here: n k-blocks from the ring into the accumulators, one k-block group in flight.
+// mma(stage) issues the wgmma of one k-block; fence() fences the accumulator registers.  A stage goes back to the producer
+// (one arrival per warp) once the group that read it has retired.  Returns the stage still held (-1 when n == 0), which
+// ring_drain releases; in between, every full-barrier wait is behind the caller (the ping-pong kernel hands over there).
+template <int STAGES, class Mma, class Fence>
+__device__ __forceinline__ int ring_mma(Ring<STAGES>& ring, uint64_t* full, uint64_t* empty, int n, Mma&& mma, Fence&& fence) {
+    const bool lane0 = (threadIdx.x & 31) == 0;
+    int prev = -1;
+    for (int kb = 0; kb < n; ++kb) {
+        mbar_wait(&full[ring.stage], ring.phase);
+        fence();
+        wgmma_fence();
+        mma(ring.stage);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
+        fence();
+        if (prev >= 0 && lane0) mbar_arrive(&empty[prev]);
+        prev = ring.stage;
+        ring.next();
+    }
+    return prev;
+}
+template <class Fence>
+__device__ __forceinline__ void ring_drain(uint64_t* empty, int held, Fence&& fence) {
+    wgmma_wait<0>();
+    fence();
+    if (held >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(&empty[held]);
+}
+
 // ---- normal mode
-constexpr int TOK_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: ping-pong consumers
+constexpr int TOK_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: consumers
+
+// Output staging of one consumer warpgroup of a token-major kernel: NS 128B-swizzled bf16 slabs of [ROWS rows][64
+// columns], one TMA store each.  A plain residual is TMA-loaded into the same slabs while the main loop runs and read
+// back in the accumulator's fragment layout with ldmatrix.
+template <int ROWS, int NS>
+struct OutSlabs {
+    static constexpr int SLAB_BYTES = ROWS * 128;
+    static constexpr int BYTES = NS * SLAB_BYTES;
+    uint8_t* p;
+    // 16-byte chunk (row, column group cg = 8 columns) as a shared-memory address
+    __device__ __forceinline__ uint32_t addr(int row, int cg) const {
+        return smem_u32(p) + (cg >> 3) * SLAB_BYTES + row * 128 + (((cg & 7) ^ (row & 7)) << 4);
+    }
+    // leader: residual rows [row0, row0 + ROWS) x the slabs' output columns from col0 that lie below n_feat
+    __device__ __forceinline__ void load_res(const CUtensorMap* map_res, uint64_t* bar, int col0, int row0, int n_feat) const {
+        bulk_wait_read<0>();  // the previous tile's store has read the slabs
+        int ns = 1;
+        while (ns < NS && col0 + 64 * ns < n_feat) ++ns;
+        mbar_arrive_expect_tx(bar, ns * SLAB_BYTES);
+        for (int s = 0; s < ns; ++s) tma_load_2d(p + s * SLAB_BYTES, map_res, bar, col0 + 64 * s, row0);
+    }
+    // whole warpgroup, before staging: the previous tile's store has read the slabs and the residual (tma_res) has landed
+    __device__ __forceinline__ void acquire(bool leader, bool tma_res, int bar_id, uint64_t* res_bar, uint32_t& res_par) const {
+        if (!tma_res && leader) bulk_wait_read<0>();
+        named_bar_sync(bar_id, 128);
+        if (tma_res) {
+            mbar_wait(res_bar, res_par);
+            res_par ^= 1;
+        }
+    }
+    // whole warpgroup, after staging: the first n slabs (those below n_feat) go out by TMA
+    __device__ __forceinline__ void store(bool leader, int bar_id, const CUtensorMap* map_out, int n, int col0, int row0, int n_feat) const {
+        fence_proxy_async_smem();
+        named_bar_sync(bar_id, 128);
+        if (leader) {
+            for (int s = 0; s < n; ++s)
+                if (col0 + 64 * s < n_feat) tma_store_2d(map_out, p + s * SLAB_BYTES, col0 + 64 * s, row0);
+            bulk_commit();
+        }
+    }
+};
+
+template <int STAGES_>
+struct TokCfg {
+    static constexpr int STAGES = STAGES_;
+    static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
+    static constexpr int STAGE_BYTES = 2 * X_BYTES;      // + 128 weight rows x 64
+    using Out = OutSlabs<128, 2>;                        // per consumer warpgroup: the 128 output columns of its tile
+    static constexpr int STAGING_BYTES = 2 * Out::BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert((2 * STAGES + 4) * 8 <= 256, "barrier area");
+    static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
+};
 // Ring depth, chosen by measurement on an H100 80GB HBM3 (700 W): 4 stages ran the prefill GEMMs 3-10 % faster than 5 (the
 // most that fits beside the 64 KB of output slabs) -- e.g. SwiGLU gate/up 24960 x 37888 x 3584 at 618-624 TFLOP/s against
 // 572-574 -- while the encoder's K = 1280 GEMMs moved by 1-4 % either way.
 constexpr int TOK_STAGES = 4;
 
-template <int STAGES>
-struct TokCfg {
+template <int STAGES_>
+struct WideCfg {
+    static constexpr int STAGES = STAGES_;
     static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
-    static constexpr int STAGE_BYTES = 2 * X_BYTES;      // + 128 weight rows x 64
-    static constexpr int SLAB_BYTES = 128 * 128;         // [128 rows][64 bf16] 128B-swizzled output / residual slab
-    static constexpr int STAGING_BYTES = 2 * 2 * SLAB_BYTES;  // per consumer warpgroup: the 128 output columns of its tile
+    static constexpr int W_BYTES = 256 * BK * 2;         // 256 weight rows x 64
+    static constexpr int STAGE_BYTES = X_BYTES + W_BYTES;
+    using Out = OutSlabs<64, 4>;                         // per consumer warpgroup: its 64 x 256 quarter of the tile
+    static constexpr int STAGING_BYTES = 2 * Out::BYTES;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert((2 * STAGES + 4) * 8 <= 256, "barrier area");
     static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
 };
+// 3 x 48 KB stages + 64 KB of staging (≈ 209 KB), chosen by measurement on an H100 80GB HBM3 (700 W): 4 stages with half
+// the staging (two epilogue passes) was as fast within run-to-run spread (prefill GEMMs -1.5 to +5 %, their time-weighted
+// sum 0.5 % slower) and needs the second pass.
+constexpr int WIDE_STAGES = 3;
 
 // ---- few-token (swap) mode
 constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma; warps 0-3 also run the epilogue), warp 8: TMA producer
@@ -159,7 +268,128 @@ __device__ __forceinline__ float epi_swiglu(float g, float u) {
     return bf16_round(s * u);
 }
 
-// ============================================================================ normal mode (n_tok > 64)
+// two consecutive bf16 of a row vector (bias / residual row) as floats; zero from column n on.  vec: p + col is 4-byte aligned
+__device__ __forceinline__ float2 ld2(const bf16* p, int col, int n, bool vec) {
+    if (vec && col + 1 < n) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + col));
+    return make_float2(col < n ? __bfloat162float(p[col]) : 0.f, col + 1 < n ? __bfloat162float(p[col + 1]) : 0.f);
+}
+
+// ============================================================================ normal mode (n_tok > 64), shared pieces
+// Shared memory of the token-major kernels: the ring (1024-byte aligned for the 128B swizzle), the output slabs of both
+// consumer warpgroups, then the barriers.
+template <class Cfg>
+struct TokSmem {
+    uint8_t* ring;
+    uint8_t* staging;
+    uint64_t* full;
+    uint64_t* empty;
+    uint64_t* rbar;   // [2] residual slabs of consumer 0 / 1 have landed
+    uint64_t* order;  // [2] ping-pong kernel only: one completion per main loop of consumer 0 / 1
+    __device__ __forceinline__ explicit TokSmem(uint8_t* raw) {
+        ring = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+        staging = ring + Cfg::STAGES * Cfg::STAGE_BYTES;
+        full = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+        empty = full + Cfg::STAGES;
+        rbar = empty + Cfg::STAGES;
+        order = rbar + 2;
+    }
+};
+
+// Thread 0 of a token-major kernel: descriptor prefetch and barrier init.  `empty` counts empty_arrivals per phase, one
+// per warp that reads the stage; the `order` barriers are initialised only when the kernel uses them.
+template <class Cfg>
+__device__ __forceinline__ void tok_prologue(const TokSmem<Cfg>& sm, uint32_t empty_arrivals, bool order, const GemmArgs& a,
+                                             const CUtensorMap* map_x, const CUtensorMap* map_w, const CUtensorMap* map_out,
+                                             const CUtensorMap* map_res, bool tma_epi, bool tma_res) {
+    trace_mark(a.trace, 0);
+    tma_prefetch_desc(map_x);
+    tma_prefetch_desc(map_w);
+    if (tma_epi) tma_prefetch_desc(map_out);
+    if (tma_res) tma_prefetch_desc(map_res);
+    for (int i = 0; i < Cfg::STAGES; ++i) {
+        mbar_init(&sm.full[i], 1);
+        mbar_init(&sm.empty[i], empty_arrivals);
+    }
+    for (int i = 0; i < 2; ++i) {
+        mbar_init(&sm.rbar[i], 1);
+        if (order) mbar_init(&sm.order[i], 1);
+    }
+    fence_barrier_init();
+}
+
+// Producer of the token-major kernels: the k-blocks of the CTA's tiles, in tile order, into the ring.  A stage holds the
+// tile's 128 token rows of X, then from X_BYTES on its weight rows, which load_w(sW, bar, k0, c) requests for column tile c.
+template <class Cfg, class LoadW>
+__device__ __forceinline__ void tok_produce(const TokSmem<Cfg>& sm, const CUtensorMap* map_x, const GemmArgs& a, LoadW&& load_w) {
+    const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+    const int kb_n = (a.K + BK - 1) / BK;
+    Ring<Cfg::STAGES> ring;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        int r, c;
+        tile_coords(t, a, r, c);
+        for (int kb = 0; kb < kb_n; ++kb) {
+            uint8_t* sX = sm.ring + ring.stage * Cfg::STAGE_BYTES;
+            uint64_t* bar = &sm.full[ring.stage];
+            mbar_wait(&sm.empty[ring.stage], ring.phase ^ 1);
+            mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
+            tma_load_2d(sX, map_x, bar, kb * BK, r * 128);
+            load_w(sX + Cfg::X_BYTES, bar, kb * BK, c);
+            ring.next();
+        }
+    }
+}
+
+// Register epilogue of the token-major kernels: one 64-row x N accumulator fragment (wgmma layout: acc[i] at row
+// 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)) through epi_elem / epi_swiglu and
+// stmatrix into slab rows [srow, srow + 64).  row0 / out_col0: the fragment's first token row and output column.
+// SwiGLU: gate in the first, up in the second half of the fragment, N / 2 output columns.
+// RES: 0 none, 1 residual already in the slabs (TMA, read back with ldmatrix), 2 rows tok % res_period from global memory.
+template <int N, int RES, class Out>
+__device__ __forceinline__ void epi_fragment(const float (&acc)[N / 2], const Out& slabs, int srow, int row0, int out_col0, int flags,
+                                          const GemmArgs& a) {
+    const int tw = threadIdx.x & 127;
+    const int warp = tw >> 5, lane = tw & 31;
+    const int frow = warp * 16 + (lane >> 2);
+    const int fcol = 2 * (lane & 3);
+    // stmatrix / ldmatrix x4 over column groups (2 n2, 2 n2 + 1) x rows (+0, +8): this lane addresses row
+    // 16 warp + 8 ((lane >> 3) & 1) + lane % 8 of the fragment, column group 2 n2 + (lane >> 4)
+    const int mrow = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+    const int mcg = lane >> 4;
+    const bool swiglu = flags & EPI_SWIGLU;
+    const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
+    const bool res_vec = (reinterpret_cast<uintptr_t>(a.resid) & 3) == 0 && (a.ld_res & 1) == 0;
+    const bf16* rp[2] = {a.resid, a.resid};
+    if constexpr (RES == 2) {
+        const int rr0 = (row0 + frow) % a.res_period;
+        rp[0] += static_cast<size_t>(rr0) * a.ld_res;
+        rp[1] += static_cast<size_t>((rr0 + 8) % a.res_period) * a.ld_res;
+    }
+#pragma unroll
+    for (int n2 = 0; n2 < (swiglu ? N / 32 : N / 16); ++n2) {
+        const uint32_t maddr = slabs.addr(srow + mrow, 2 * n2 + mcg);
+        uint32_t rr[4];
+        if constexpr (RES == 1) ldmatrix_x4(maddr, rr);  // residual pairs in the accumulator's fragment layout
+        uint32_t y[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int cg = 2 * n2 + (q >> 1);  // column group; q & 1: rows +0 / +8
+            const int i = 4 * cg + 2 * (q & 1);
+            if (swiglu) {
+                y[q] = pack_bf16x2(epi_swiglu(acc[i], acc[i + N / 4]), epi_swiglu(acc[i + 1], acc[i + N / 4 + 1]));
+            } else {
+                const int col = out_col0 + 8 * cg + fcol;
+                const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, a.n_feat, bias_vec) : make_float2(0.f, 0.f);
+                float2 res = make_float2(0.f, 0.f);
+                if constexpr (RES == 1) res = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rr[q]));
+                if constexpr (RES == 2) res = ld2(rp[q & 1], col, a.n_feat, res_vec);
+                y[q] = pack_bf16x2(epi_elem(acc[i], flags, b.x, res.x), epi_elem(acc[i + 1], flags, b.y, res.y));
+            }
+        }
+        stmatrix_x4(maddr, y[0], y[1], y[2], y[3]);
+    }
+}
+
+// ============================================================================ normal mode, 128 x 128 ping-pong tiles
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches); EPI < 0: generic instantiation reading
 // a.flags at run time (odd layouts / unusual flag mixes).
 //
@@ -175,12 +405,7 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
     using Cfg = TokCfg<STAGES>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* order = empty + STAGES;  // [2] one completion per main loop of consumer 0 / 1
-    uint64_t* rbar = order + 2;        // [2] residual slabs of consumer 0 / 1 have landed
+    const TokSmem<Cfg> sm(smem_raw);
 
     const int wg = threadIdx.x >> 7;
     const int tw = threadIdx.x & 127;
@@ -188,87 +413,35 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     const bool swiglu = flags & EPI_SWIGLU;
     const bool tma_res = a.tma_epi && (flags & EPI_RESID) && a.res_period == 0;
 
-    if (threadIdx.x == 0) {
-        trace_mark(a.trace, 0);
-        tma_prefetch_desc(&map_x);
-        tma_prefetch_desc(&map_w);
-        for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 4);  // one arrival per warp of the consuming warpgroup
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&order[i], 1);
-            mbar_init(&rbar[i], 1);
-        }
-        if (a.tma_epi) {
-            tma_prefetch_desc(&map_out);
-            if (tma_res) tma_prefetch_desc(&map_res);
-        }
-        fence_barrier_init();
-    }
+    // `empty`: 4 arrivals, one per warp of the warpgroup that consumes the tile; `order` barriers for the ping-pong
+    if (threadIdx.x == 0) tok_prologue(sm, 4, true, a, &map_x, &map_w, &map_out, &map_res, a.tma_epi, tma_res);
     __syncthreads();
     pdl_launch_dependents();  // the next kernel may start its prologue behind us
-
-    const int num_tiles = a.num_r_tiles * a.num_c_tiles;
-    const int kb_n = (a.K + BK - 1) / BK;
 
     if (wg == 0) {
         setmaxnreg_dec<40>();
         if (tw == 0) {
-            // SwiGLU tile c (output features [64c, 64c + 64)): the 64 gate rows, then the 64 up rows of the same features --
-            // 128 rows later (gate / up interleaved in blocks of 128 rows) or at swiglu_up_row0 + 64c ([gate; up])
-            auto gate_row = [&](int c) { return a.swiglu_up_row0 ? c * 64 : (c >> 1) * 256 + (c & 1) * 64; };
-            auto up_row = [&](int c) { return a.swiglu_up_row0 ? a.swiglu_up_row0 + c * 64 : gate_row(c) + 128; };
             pdl_wait();
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                int r, c;
-                tile_coords(t, a, r, c);
-                for (int kb = 0; kb < kb_n; ++kb) {
-                    uint8_t* sX = smem + stage * Cfg::STAGE_BYTES;
-                    uint8_t* sW = sX + Cfg::X_BYTES;
-                    mbar_wait(&empty[stage], phase ^ 1);
-                    mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-                    tma_load_2d(sX, &map_x, &full[stage], kb * BK, r * 128);
-                    if (swiglu) {
-                        tma_load_2d(sW, &map_w, &full[stage], kb * BK, gate_row(c));
-                        tma_load_2d(sW + 64 * BK * 2, &map_w, &full[stage], kb * BK, up_row(c));
-                    } else {
-                        tma_load_2d(sW, &map_w, &full[stage], kb * BK, c * 128);
-                    }
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
+            tok_produce(sm, &map_x, a, [&](uint8_t* sW, uint64_t* bar, int k0, int c) {
+                if (swiglu) {
+                    // SwiGLU tile c (output features [64c, 64c + 64)): the 64 gate rows, then the 64 up rows of the same
+                    // features -- 128 rows later (gate / up interleaved in blocks of 128 rows) or at swiglu_up_row0 + 64c ([gate; up])
+                    const int gate_row = a.swiglu_up_row0 ? c * 64 : (c >> 1) * 256 + (c & 1) * 64;
+                    const int up_row = a.swiglu_up_row0 ? a.swiglu_up_row0 + c * 64 : gate_row + 128;
+                    tma_load_2d(sW, &map_w, bar, k0, gate_row);
+                    tma_load_2d(sW + 64 * BK * 2, &map_w, bar, k0, up_row);
+                } else {
+                    tma_load_2d(sW, &map_w, bar, k0, c * 128);
                 }
-            }
+            });
         }
     } else {
         setmaxnreg_inc<232>();
         const int cw = wg - 1;  // consumer index
-        const int warp = tw >> 5, lane = tw & 31;
-        uint8_t* stg = staging + cw * 2 * Cfg::SLAB_BYTES;
-        const uint32_t stg_u32 = smem_u32(stg);
         const bool leader = tw == 0;
-        const int n_slabs = swiglu ? 1 : 2;  // 64-column output slabs per tile
-        // accumulator fragment acc[h][i]: tile row h * 64 + 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
-        const int frow = warp * 16 + (lane >> 2);
-        const int fcol = 2 * (lane & 3);
-        // stmatrix / ldmatrix x4 over column groups (2 n2, 2 n2 + 1) x rows (+0, +8): this lane addresses row
-        // 16 warp + 8 ((lane >> 3) & 1) + lane % 8 of the 64-row half, column group 2 n2 + (lane >> 4)
-        const int mrow = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-        const int mcg = lane >> 4;
-        auto slab_addr = [&](int row, int cg) {  // 16-byte chunk (row, column group cg of the tile) in the swizzled slabs
-            return stg_u32 + (cg >> 3) * Cfg::SLAB_BYTES + row * 128 + (((cg & 7) ^ (row & 7)) << 4);
-        };
-        const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
-        const bool res_vec = (reinterpret_cast<uintptr_t>(a.resid) & 3) == 0 && (a.ld_res & 1) == 0;
-        // two consecutive bf16 of a row vector (bias / residual row) as floats; zero past n
-        auto ld2 = [&](const bf16* p, int col, bool vec) {
-            if (vec && col + 1 < a.n_feat) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + col));
-            return make_float2(col < a.n_feat ? __bfloat162float(p[col]) : 0.f, col + 1 < a.n_feat ? __bfloat162float(p[col + 1]) : 0.f);
-        };
+        const typename Cfg::Out slabs{sm.staging + cw * Cfg::Out::BYTES};
+        const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+        const int kb_n = (a.K + BK - 1) / BK;
         pdl_wait();  // residual reads / output writes are ordered after every earlier kernel
         if (threadIdx.x == 128) trace_mark(a.trace, 1);
         uint32_t rpar = 0;
@@ -278,12 +451,8 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             int r, c;
             tile_coords(t, a, r, c);
             const int out_col0 = c * (swiglu ? 64 : 128);
-            if (tma_res && leader) {  // residual slabs of this tile: they arrive while the main loop runs
-                bulk_wait_read<0>();  // the previous tile's store has read the staging slabs
-                const int ns = (out_col0 + 64 < a.n_feat) ? 2 : 1;
-                mbar_arrive_expect_tx(&rbar[cw], ns * Cfg::SLAB_BYTES);
-                for (int s = 0; s < ns; ++s) tma_load_2d(stg + s * Cfg::SLAB_BYTES, &map_res, &rbar[cw], out_col0 + 64 * s, r * 128);
-            }
+            // residual slabs of this tile: they arrive while the main loop runs
+            if (tma_res && leader) slabs.load_res(&map_res, &sm.rbar[cw], out_col0, r * 128, a.n_feat);
 
             // ---- main loop: 128 x 128 tile, two m64n128k16 per k16 step (rows 0-63, rows 64-127)
             float acc[2][64];
@@ -291,18 +460,15 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
             for (int h = 0; h < 2; ++h)
 #pragma unroll
                 for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
-            if (j > 0) mbar_wait(&order[cw ^ 1], ((j - 1) >> 1) & 1);  // tile j - 1 fully issued by the other consumer
-            const int g0 = j * kb_n;  // ring slot of this tile's first k-block
-            int stage = g0 % STAGES;
-            uint32_t phase = (g0 / STAGES) & 1;
-            int prev = -1;
-            for (int kb = 0; kb < kb_n; ++kb) {
-                mbar_wait(&full[stage], phase);
-                const uint32_t sX = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                const uint32_t sW = sX + Cfg::X_BYTES;
+            if (j > 0) mbar_wait(&sm.order[cw ^ 1], ((j - 1) >> 1) & 1);  // tile j - 1 fully issued by the other consumer
+            Ring<STAGES> ring(j * kb_n);  // ring slot of this tile's first k-block
+            auto fence = [&] {
                 fence_regs(acc[0]);
                 fence_regs(acc[1]);
-                wgmma_fence();
+            };
+            const int held = ring_mma(ring, sm.full, sm.empty, kb_n, [&](int stage) {
+                const uint32_t sX = smem_u32(sm.ring + stage * Cfg::STAGE_BYTES);
+                const uint32_t sW = sX + Cfg::X_BYTES;
 #pragma unroll
                 for (int k = 0; k < BK / 16; ++k) {
                     const uint64_t bdesc = make_smem_desc_sw128(sW + k * 32, 0, 1024);
@@ -310,69 +476,21 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                     for (int h = 0; h < 2; ++h)
                         wgmma_m64n128_ss<0, 0>(acc[h], make_smem_desc_sw128(sX + h * 64 * 128 + k * 32, 0, 1024), bdesc, 1);
                 }
-                wgmma_commit();
-                wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
-                fence_regs(acc[0]);
-                fence_regs(acc[1]);
-                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-                prev = stage;
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            if (leader) mbar_arrive(&order[cw]);  // every full-barrier wait of this tile is behind us: the other consumer may start
-            wgmma_wait<0>();
-            fence_regs(acc[0]);
-            fence_regs(acc[1]);
-            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            }, fence);
+            if (leader) mbar_arrive(&sm.order[cw]);  // every full-barrier wait of this tile is behind us: the other consumer may start
+            ring_drain(sm.empty, held, fence);
             if (threadIdx.x == 128) trace_mark(a.trace, 2);
 
             // ---- epilogue from the accumulator fragments
-            // the compile-time epilogues are launched only with the TMA-store path (launch_normal); the direct-store fallback
+            // the compile-time epilogues are launched only with the TMA-store path (gemm_bf16); the direct-store fallback
             // exists in the generic instantiation alone, which keeps the specialised kernels small
             if (EPI >= 0 || a.tma_epi) {
-                if (!tma_res && leader) bulk_wait_read<0>();
-                named_bar_sync(1 + cw, 128);  // the previous tile's store has read the staging slabs
-                if (tma_res) {
-                    mbar_wait(&rbar[cw], rpar);
-                    rpar ^= 1;
-                }
+                slabs.acquire(leader, tma_res, 1 + cw, &sm.rbar[cw], rpar);
                 // one unrolled pass over the tile per residual source, so that each pass holds only its own operands
-                auto stage_tile = [&](auto res_src) {  // 0: none, 1: slab in smem (TMA), 2: periodic rows from global memory
+                auto stage_tile = [&](auto res_src) {
                     constexpr int RES = decltype(res_src)::value;
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const bf16* rp[2] = {a.resid, a.resid};
-                        if constexpr (RES == 2) {
-                            const int rr0 = (r * 128 + h * 64 + frow) % a.res_period;
-                            rp[0] += static_cast<size_t>(rr0) * a.ld_res;
-                            rp[1] += static_cast<size_t>((rr0 + 8) % a.res_period) * a.ld_res;
-                        }
-#pragma unroll
-                        for (int n2 = 0; n2 < (swiglu ? 4 : 8); ++n2) {
-                            const uint32_t maddr = slab_addr(h * 64 + mrow, 2 * n2 + mcg);
-                            uint32_t rr[4];
-                            if constexpr (RES == 1) ldmatrix_x4(maddr, rr);  // residual pairs in the accumulator's fragment layout
-                            uint32_t y[4];
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                const int cg = 2 * n2 + (q >> 1);  // column group; q & 1: rows +0 / +8
-                                const int i = 4 * cg + 2 * (q & 1);
-                                if (swiglu) {
-                                    y[q] = pack_bf16x2(epi_swiglu(acc[h][i], acc[h][i + 32]), epi_swiglu(acc[h][i + 1], acc[h][i + 33]));
-                                } else {
-                                    const int col = out_col0 + 8 * cg + fcol;
-                                    const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, bias_vec) : make_float2(0.f, 0.f);
-                                    float2 res = make_float2(0.f, 0.f);
-                                    if constexpr (RES == 1) res = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rr[q]));
-                                    if constexpr (RES == 2) res = ld2(rp[q & 1], col, res_vec);
-                                    y[q] = pack_bf16x2(epi_elem(acc[h][i], flags, b.x, res.x), epi_elem(acc[h][i + 1], flags, b.y, res.y));
-                                }
-                            }
-                            stmatrix_x4(maddr, y[0], y[1], y[2], y[3]);
-                        }
-                    }
+                    epi_fragment<128, RES>(acc[0], slabs, 0, r * 128, out_col0, flags, a);
+                    epi_fragment<128, RES>(acc[1], slabs, 64, r * 128 + 64, out_col0, flags, a);
                 };
                 if (tma_res)
                     stage_tile(IntC<1>{});
@@ -380,15 +498,14 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                     stage_tile(IntC<2>{});
                 else
                     stage_tile(IntC<0>{});
-                fence_proxy_async_smem();
-                named_bar_sync(1 + cw, 128);
-                if (leader) {
-                    for (int s = 0; s < n_slabs; ++s)
-                        if (out_col0 + 64 * s < a.n_feat) tma_store_2d(&map_out, stg + s * Cfg::SLAB_BYTES, out_col0 + 64 * s, r * 128);
-                    bulk_commit();
-                }
+                slabs.store(leader, 1 + cw, &map_out, swiglu ? 1 : 2, out_col0, r * 128, a.n_feat);
             } else {
                 // direct stores (output rows not 16-byte aligned, fp32 output): element pairs straight from the fragments
+                const int warp = tw >> 5, lane = tw & 31;
+                const int frow = warp * 16 + (lane >> 2);
+                const int fcol = 2 * (lane & 3);
+                const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
+                const bool res_vec = (reinterpret_cast<uintptr_t>(a.resid) & 3) == 0 && (a.ld_res & 1) == 0;
                 const bool out_vec = (reinterpret_cast<uintptr_t>(a.out) & ((flags & EPI_F32OUT) ? 7 : 3)) == 0 && (a.ldo & 1) == 0;
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -406,9 +523,10 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                             if (swiglu) {
                                 v = make_float2(epi_swiglu(acc[h][i], acc[h][i + 32]), epi_swiglu(acc[h][i + 1], acc[h][i + 33]));
                             } else {
-                                const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, bias_vec) : make_float2(0.f, 0.f);
-                                const float2 res = (flags & EPI_RESID) ? ld2(a.resid + static_cast<size_t>(res_row) * a.ld_res, col, res_vec)
-                                                                       : make_float2(0.f, 0.f);
+                                const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col, a.n_feat, bias_vec) : make_float2(0.f, 0.f);
+                                const float2 res = (flags & EPI_RESID)
+                                                       ? ld2(a.resid + static_cast<size_t>(res_row) * a.ld_res, col, a.n_feat, res_vec)
+                                                       : make_float2(0.f, 0.f);
                                 v = make_float2(epi_elem(acc[h][i], flags, b.x, res.x), epi_elem(acc[h][i + 1], flags, b.y, res.y));
                             }
                             const size_t o = static_cast<size_t>(tok) * a.ldo + col;
@@ -449,22 +567,6 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
 // holds gate (acc[i]) and up (acc[i + 64]) of its outputs.  The two consumers finish a tile together, so the epilogue is
 // not hidden behind a main loop; the producer runs ahead into the next tile meanwhile.  Staging: the whole 64 x 256
 // quarter of each consumer (4 slabs of [64 rows x 64 columns]); a plain residual is TMA-loaded into it during the main loop.
-template <int STAGES>
-struct WideCfg {
-    static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
-    static constexpr int W_BYTES = 256 * BK * 2;         // 256 weight rows x 64
-    static constexpr int STAGE_BYTES = X_BYTES + W_BYTES;
-    static constexpr int SLAB_BYTES = 64 * 128;          // [64 rows][64 bf16] 128B-swizzled output / residual slab
-    static constexpr int STAGING_BYTES = 2 * 4 * SLAB_BYTES;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-    static_assert((2 * STAGES + 2) * 8 <= 256, "barrier area");
-    static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
-};
-// 3 x 48 KB stages + 64 KB of staging (≈ 209 KB), chosen by measurement on an H100 80GB HBM3 (700 W): 4 stages with half
-// the staging (two epilogue passes) was as fast within run-to-run spread (prefill GEMMs -1.5 to +5 %, their time-weighted
-// sum 0.5 % slower) and needs the second pass.
-constexpr int WIDE_STAGES = 3;
-
 template <int STAGES, int EPI>
 __global__ void __launch_bounds__(TOK_THREADS, 1)
 gemm_tok_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
@@ -472,11 +574,7 @@ gemm_tok_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     static_assert(EPI >= 0 && !(EPI & EPI_F32OUT), "compile-time epilogue with a TMA store");
     using Cfg = WideCfg<STAGES>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* rbar = empty + STAGES;  // [2] residual slabs of consumer 0 / 1 have landed
+    const TokSmem<Cfg> sm(smem_raw);
 
     const int wg = threadIdx.x >> 7;
     const int tw = threadIdx.x & 127;
@@ -485,158 +583,60 @@ gemm_tok_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     constexpr int OUT_COLS = swiglu ? 128 : 256;  // output columns of a tile
     constexpr bool tma_res = flags & EPI_RESID;  // plain residual only (the host keeps periodic ones on the 128 x 128 kernel)
 
-    if (threadIdx.x == 0) {
-        trace_mark(a.trace, 0);
-        tma_prefetch_desc(&map_x);
-        tma_prefetch_desc(&map_w);
-        tma_prefetch_desc(&map_out);
-        if (tma_res) tma_prefetch_desc(&map_res);
-        for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 8);  // one arrival per consumer warp: both warpgroups read every stage
-        }
-        for (int i = 0; i < 2; ++i) mbar_init(&rbar[i], 1);
-        fence_barrier_init();
-    }
+    // `empty`: 8 arrivals, one per consumer warp, since both warpgroups read every stage; no `order` barriers
+    if (threadIdx.x == 0) tok_prologue(sm, 8, false, a, &map_x, &map_w, &map_out, &map_res, true, tma_res);
     __syncthreads();
     pdl_launch_dependents();  // the next kernel may start its prologue behind us
-
-    const int num_tiles = a.num_r_tiles * a.num_c_tiles;
-    const int kb_n = (a.K + BK - 1) / BK;
 
     if (wg == 0) {
         setmaxnreg_dec<40>();
         if (tw == 0) {
-            // weight rows of 128-row half q of column tile c
-            auto w_row = [&](int c, int q) {
-                if (swiglu && a.swiglu_up_row0) return q ? a.swiglu_up_row0 + c * 128 : c * 128;  // [gate; up]
-                return c * 256 + q * 128;  // plain, or one 256-row block of the gate / up interleaved layout
-            };
             pdl_wait();
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-                int r, c;
-                tile_coords(t, a, r, c);
-                for (int kb = 0; kb < kb_n; ++kb) {
-                    uint8_t* sX = smem + stage * Cfg::STAGE_BYTES;
-                    uint8_t* sW = sX + Cfg::X_BYTES;
-                    mbar_wait(&empty[stage], phase ^ 1);
-                    mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-                    tma_load_2d(sX, &map_x, &full[stage], kb * BK, r * 128);
-                    tma_load_2d(sW, &map_w, &full[stage], kb * BK, w_row(c, 0));
-                    tma_load_2d(sW + Cfg::W_BYTES / 2, &map_w, &full[stage], kb * BK, w_row(c, 1));
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-            }
+            tok_produce(sm, &map_x, a, [&](uint8_t* sW, uint64_t* bar, int k0, int c) {
+                // the two 128-row halves: plain, or one 256-row block of the gate / up interleaved layout, or gate and up of [gate; up]
+                const bool concat = swiglu && a.swiglu_up_row0;
+                tma_load_2d(sW, &map_w, bar, k0, concat ? c * 128 : c * 256);
+                tma_load_2d(sW + Cfg::W_BYTES / 2, &map_w, bar, k0, concat ? a.swiglu_up_row0 + c * 128 : c * 256 + 128);
+            });
         }
     } else {
         setmaxnreg_inc<232>();
         const int cw = wg - 1;  // consumer index: token rows [64 cw, 64 cw + 64) of the tile
-        const int warp = tw >> 5, lane = tw & 31;
-        uint8_t* stg = staging + cw * 4 * Cfg::SLAB_BYTES;
-        const uint32_t stg_u32 = smem_u32(stg);
         const bool leader = tw == 0;
-        // accumulator fragment acc[i]: row 16 warp + lane / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
-        const int fcol = 2 * (lane & 3);
-        // stmatrix / ldmatrix x4 over column groups (2 n2, 2 n2 + 1) x rows (+0, +8): this lane addresses row
-        // 16 warp + 8 ((lane >> 3) & 1) + lane % 8, column group 2 n2 + (lane >> 4)
-        const int mrow = warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
-        const int mcg = lane >> 4;
-        auto slab_addr = [&](int row, int cg) {  // 16-byte chunk (row, column group cg) in the swizzled slabs
-            return stg_u32 + (cg >> 3) * Cfg::SLAB_BYTES + row * 128 + (((cg & 7) ^ (row & 7)) << 4);
-        };
-        const bool bias_vec = (reinterpret_cast<uintptr_t>(a.bias) & 3) == 0;
-        auto ld2 = [&](const bf16* p, int col) {  // two consecutive bias values as floats; zero past n_feat
-            if (bias_vec && col + 1 < a.n_feat) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + col));
-            return make_float2(col < a.n_feat ? __bfloat162float(p[col]) : 0.f, col + 1 < a.n_feat ? __bfloat162float(p[col + 1]) : 0.f);
-        };
+        const typename Cfg::Out slabs{sm.staging + cw * Cfg::Out::BYTES};
+        const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+        const int kb_n = (a.K + BK - 1) / BK;
         pdl_wait();  // residual reads / output writes are ordered after every earlier kernel
         if (threadIdx.x == 128) trace_mark(a.trace, 1);
         uint32_t rpar = 0;
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring<STAGES> ring;
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
             int r, c;
             tile_coords(t, a, r, c);
             const int row0 = r * 128 + cw * 64;  // first token row of this warpgroup
             const int out_col0 = c * OUT_COLS;
-            if (tma_res && leader) {  // residual slabs of this tile: they arrive while the main loop runs
-                bulk_wait_read<0>();  // the previous tile's store has read the staging slabs
-                int ns = 0;
-                while (ns < 4 && out_col0 + 64 * ns < a.n_feat) ++ns;
-                mbar_arrive_expect_tx(&rbar[cw], ns * Cfg::SLAB_BYTES);
-                for (int s = 0; s < ns; ++s) tma_load_2d(stg + s * Cfg::SLAB_BYTES, &map_res, &rbar[cw], out_col0 + 64 * s, row0);
-            }
+            // residual slabs of this tile: they arrive while the main loop runs
+            if (tma_res && leader) slabs.load_res(&map_res, &sm.rbar[cw], out_col0, row0, a.n_feat);
 
             // ---- main loop: one m64n256k16 per k16 step
             float acc[128];
 #pragma unroll
             for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-            int prev = -1;
-            for (int kb = 0; kb < kb_n; ++kb) {
-                mbar_wait(&full[stage], phase);
-                const uint32_t sX = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 64 * 128;
-                const uint32_t sW = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::X_BYTES;
-                fence_regs(acc);
-                wgmma_fence();
+            auto fence = [&] { fence_regs(acc); };
+            const int held = ring_mma(ring, sm.full, sm.empty, kb_n, [&](int stage) {
+                const uint32_t sX = smem_u32(sm.ring + stage * Cfg::STAGE_BYTES) + cw * 64 * 128;
+                const uint32_t sW = smem_u32(sm.ring + stage * Cfg::STAGE_BYTES) + Cfg::X_BYTES;
 #pragma unroll
                 for (int k = 0; k < BK / 16; ++k)
                     wgmma_m64n256_ss<0, 0>(acc, make_smem_desc_sw128(sX + k * 32, 0, 1024), make_smem_desc_sw128(sW + k * 32, 0, 1024), 1);
-                wgmma_commit();
-                wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
-                fence_regs(acc);
-                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-                prev = stage;
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            wgmma_wait<0>();
-            fence_regs(acc);
-            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            }, fence);
+            ring_drain(sm.empty, held, fence);
             if (threadIdx.x == 128) trace_mark(a.trace, 2);
 
             // ---- epilogue from the accumulator fragments
-            if (!tma_res && leader) bulk_wait_read<0>();
-            named_bar_sync(1 + cw, 128);  // the previous tile's store has read the staging slabs
-            if (tma_res) {
-                mbar_wait(&rbar[cw], rpar);
-                rpar ^= 1;
-            }
-#pragma unroll
-            for (int n2 = 0; n2 < OUT_COLS / 16; ++n2) {
-                const uint32_t maddr = slab_addr(mrow, 2 * n2 + mcg);
-                uint32_t rr[4];
-                if constexpr (tma_res) ldmatrix_x4(maddr, rr);  // residual pairs in the accumulator's fragment layout
-                uint32_t y[4];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int cg = 2 * n2 + (q >> 1);  // column group; q & 1: rows +0 / +8
-                    const int i = 4 * cg + 2 * (q & 1);
-                    if constexpr (swiglu) {
-                        y[q] = pack_bf16x2(epi_swiglu(acc[i], acc[i + 64]), epi_swiglu(acc[i + 1], acc[i + 65]));
-                    } else {
-                        const int col = out_col0 + 8 * cg + fcol;
-                        const float2 b = (flags & EPI_BIAS) ? ld2(a.bias, col) : make_float2(0.f, 0.f);
-                        float2 res = make_float2(0.f, 0.f);
-                        if constexpr (tma_res) res = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rr[q]));
-                        y[q] = pack_bf16x2(epi_elem(acc[i], flags, b.x, res.x), epi_elem(acc[i + 1], flags, b.y, res.y));
-                    }
-                }
-                stmatrix_x4(maddr, y[0], y[1], y[2], y[3]);
-            }
-            fence_proxy_async_smem();
-            named_bar_sync(1 + cw, 128);
-            if (leader) {
-                for (int s = 0; s < OUT_COLS / 64; ++s)
-                    if (out_col0 + 64 * s < a.n_feat) tma_store_2d(&map_out, stg + s * Cfg::SLAB_BYTES, out_col0 + 64 * s, row0);
-                bulk_commit();
-            }
+            slabs.acquire(leader, tma_res, 1 + cw, &sm.rbar[cw], rpar);
+            epi_fragment<256, tma_res ? 1 : 0>(acc, slabs, 0, row0, out_col0, flags, a);
+            slabs.store(leader, 1 + cw, &map_out, OUT_COLS / 64, out_col0, row0, a.n_feat);
         }
         if (leader) bulk_wait_read<0>();  // staged tiles must be read out before shared memory goes away
     }
@@ -684,8 +684,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 
     if (warp == 8) {
         if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
+            Ring<STAGES> ring;
             // The row operand is a WEIGHT matrix, independent of earlier kernels -> its first STAGES tiles are
             // requested before pdl_wait(), so weight streaming overlaps the tail of the previous kernel(s).
             int prefetched = 0;
@@ -712,21 +711,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                 tile_coords(t / k_splits, a, r, c);
                 const int sp = t % k_splits;
                 for (int kb = kb_lo(sp); kb < kb_lo(sp + 1); ++kb, ++issued) {
-                    uint8_t* sR = smem + stage * Cfg::STAGE_BYTES;
+                    uint8_t* sR = smem + ring.stage * Cfg::STAGE_BYTES;
                     uint8_t* sC = sR + Cfg::R_BYTES;
                     if (issued >= prefetched) {
-                        mbar_wait(&empty[stage], phase ^ 1);
-                        mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+                        mbar_wait(&empty[ring.stage], ring.phase ^ 1);
+                        mbar_arrive_expect_tx(&full[ring.stage], Cfg::STAGE_BYTES);
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
-                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[stage], kb * BK,
+                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[ring.stage], kb * BK,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
-                    tma_load_2d(sC, &map_c, &full[stage], kb * BK, c * BN);
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
+                    tma_load_2d(sC, &map_c, &full[ring.stage], kb * BK, c * BN);
+                    ring.next();
                 }
             }
         }
@@ -741,25 +737,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
         const bool epi_warp = warp < 4;
         pdl_wait();  // residual reads / output writes / split-K workspace are ordered after every earlier kernel
         if (threadIdx.x == 0) trace_mark(a.trace, 1);
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring<STAGES> ring;
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
             {
                 const int sp = t % k_splits;
-                const int kb0 = kb_lo(sp), kb1 = kb_lo(sp + 1);
                 float accr[NA][BN / 2];
 #pragma unroll
                 for (int na = 0; na < NA; ++na)
 #pragma unroll
                     for (int i = 0; i < BN / 2; ++i) accr[na][i] = 0.f;
-                int prev = -1;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(&full[stage], phase);
-                    const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t sC = sR + Cfg::R_BYTES;
+                auto fence = [&] {
 #pragma unroll
                     for (int na = 0; na < NA; ++na) fence_regs(accr[na]);
-                    wgmma_fence();
+                };
+                const int held = ring_mma(ring, full, empty, kb_lo(sp + 1) - kb_lo(sp), [&](int stage) {
+                    const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+                    const uint32_t sC = sR + Cfg::R_BYTES;
 #pragma unroll
                     for (int k = 0; k < BK / 16; ++k) {
                         const uint64_t bdesc = make_smem_desc_sw128(sC + k * 32, 0, 1024);
@@ -769,21 +762,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                             wgmma_m64n32_ss<0, 0>(accr[na], adesc, bdesc, 1);
                         }
                     }
-                    wgmma_commit();
-                    wgmma_wait<1>();  // the previous k-block's group has retired: its stage goes back to the producer
-#pragma unroll
-                    for (int na = 0; na < NA; ++na) fence_regs(accr[na]);
-                    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-                    prev = stage;
-                    if (++stage == STAGES) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                wgmma_wait<0>();
-#pragma unroll
-                for (int na = 0; na < NA; ++na) fence_regs(accr[na]);
-                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                }, fence);
+                ring_drain(empty, held, fence);
                 asm volatile("bar.sync 3, 256;" ::: "memory");  // the previous tile's epilogue is done with accbuf
 #pragma unroll
                 for (int na = 0; na < NA; ++na)
@@ -801,7 +781,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             // (the epilogue otherwise exposes one more L2 round trip in the split-K tail)
             [[maybe_unused]] uint4 rv_pre[4];
             [[maybe_unused]] bool rv_ok = false;
-            if constexpr (BN == 32 && NA == 1) {
+            if constexpr (NA == 1) {
                 if ((flags & EPI_RESID) && !(flags & EPI_F32OUT) && (a.ldo & 7) == 0 && (a.ld_res & 7) == 0 && a.res_period == 0) {
                     const int et = threadIdx.x;
                     const int tok = c * BN + (et >> 2);
@@ -821,184 +801,179 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                 const int feat = r * 128 + row_in_tile;
                 const bool feat_ok = feat < a.n_feat;
                 const float bias = ((flags & EPI_BIAS) && feat_ok) ? __bfloat162float(a.bias[feat]) : 0.f;
-#pragma unroll 1
-                for (int ch = 0; ch < BN / 32; ++ch) {
-                    uint32_t v[32], u[32];
-                    acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, ch * 32, v);
-                    if constexpr (NA == 2) acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, BN + ch * 32, u);
-                    if constexpr (NA == 1 && BN == 32) {
-                        if (k_splits > 1) {
-                            // publish this split's partial tile: ws[tile][split][col][row] (row fastest: coalesced)
-                            const int tile = t / k_splits, sp = t % k_splits;
-                            float* wt = a.ws + (static_cast<size_t>(tile) * k_splits) * (BN * 128);
+                uint32_t v[32], u[32];
+                acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, 0, v);
+                if constexpr (NA == 2) acc_ld32<Cfg::ACC_COLS>(accbuf, row_in_tile, BN, u);
+                if constexpr (NA == 1) {
+                    if (k_splits > 1) {
+                        // publish this split's partial tile: ws[tile][split][col][row] (row fastest: coalesced)
+                        const int tile = t / k_splits, sp = t % k_splits;
+                        float* wt = a.ws + (static_cast<size_t>(tile) * k_splits) * (BN * 128);
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) wt[(sp * BN + j) * 128 + row_in_tile] = __uint_as_float(v[j]);
-                            // release: the barrier orders every thread's partial stores before thread 64's fence + counter
-                            // increment (fences are cumulative -- the cooperative-groups grid-sync pattern); acquire: thread 64's
-                            // fence after the increment, then the barrier, then L2 (.cg) loads by everyone
-                            asm volatile("bar.sync 1, 128;" ::: "memory");
-                            if (threadIdx.x == 0) {
-                                __threadfence();
-                                const int arrived_now = atomicAdd(a.counters + tile, 1);
-                                __threadfence();
-                                *reinterpret_cast<volatile int*>(flag_slot) = arrived_now;
-                            }
-                            asm volatile("bar.sync 1, 128;" ::: "memory");
-                            const int arrived = *reinterpret_cast<volatile int*>(flag_slot);
-                            if (arrived != k_splits - 1) continue;  // not the last split of this tile: done
-                            // Sum in split order (deterministic: 0, 1, 2, ...).  Two register buffers keep the loads of split s + 1
-                            // (and s + 2) in flight while split s is added: k_splits dependent L2 round trips become ~k_splits / 2.
-                            float sum[32], ta[32], tb[32];
-                            auto ld_part = [&](float (&d)[32], int s2) {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) d[j] = __ldcg(wt + (s2 * BN + j) * 128 + row_in_tile);
-                            };
-                            ld_part(ta, 0);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) sum[j] = 0.f;
-                            for (int s2 = 0; s2 < k_splits; s2 += 2) {
-                                if (s2 + 1 < k_splits) ld_part(tb, s2 + 1);
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) sum[j] += ta[j];
-                                if (s2 + 2 < k_splits) ld_part(ta, s2 + 2);
-                                if (s2 + 1 < k_splits) {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j) sum[j] += tb[j];
-                                }
-                            }
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(sum[j]);
-                            if (threadIdx.x == 0) a.counters[tile] = 0;
+                        for (int j = 0; j < 32; ++j) wt[(sp * BN + j) * 128 + row_in_tile] = __uint_as_float(v[j]);
+                        // release: the barrier orders every thread's partial stores before thread 64's fence + counter
+                        // increment (fences are cumulative -- the cooperative-groups grid-sync pattern); acquire: thread 64's
+                        // fence after the increment, then the barrier, then L2 (.cg) loads by everyone
+                        asm volatile("bar.sync 1, 128;" ::: "memory");
+                        if (threadIdx.x == 0) {
+                            __threadfence();
+                            const int arrived_now = atomicAdd(a.counters + tile, 1);
+                            __threadfence();
+                            *reinterpret_cast<volatile int*>(flag_slot) = arrived_now;
                         }
-                    }
-                    const int tok0 = c * BN + ch * 32;
-                    if constexpr (BN == 32) {
-                        if (!(flags & EPI_F32OUT) && (a.ldo & 7) == 0 && (!(flags & EPI_RESID) || ((a.ld_res & 7) == 0 && a.res_period == 0))) {
-                            // ---- transposed epilogue: this thread owns feature `feat` for 32 tokens, but the output (and the
-                            // residual) are token-major.  Pre-residual values go through a [32 tok][128 feat] bf16 smem tile so
-                            // that global traffic is 16-byte vectors along the feature dimension (4 loads + 4 stores per thread
-                            // instead of 32 + 32 scalar ones whose latencies ptxas otherwise serialises).
-                            bf16* tile = reinterpret_cast<bf16*>(epi_stage);
+                        asm volatile("bar.sync 1, 128;" ::: "memory");
+                        const int arrived = *reinterpret_cast<volatile int*>(flag_slot);
+                        if (arrived != k_splits - 1) continue;  // not the last split of this tile: done
+                        // Sum in split order (deterministic: 0, 1, 2, ...).  Two register buffers keep the loads of split s + 1
+                        // (and s + 2) in flight while split s is added: k_splits dependent L2 round trips become ~k_splits / 2.
+                        float sum[32], ta[32], tb[32];
+                        auto ld_part = [&](float (&d)[32], int s2) {
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                float y;
-                                if constexpr (NA == 2)
-                                    y = epi_swiglu(__uint_as_float(v[j]), __uint_as_float(u[j]));
-                                else
-                                    y = epi_elem(__uint_as_float(v[j]), flags & ~EPI_RESID, bias, 0.f);
-                                tile[j * 128 + row_in_tile] = __float2bfloat16_rn(y);
+                            for (int j = 0; j < 32; ++j) d[j] = __ldcg(wt + (s2 * BN + j) * 128 + row_in_tile);
+                        };
+                        ld_part(ta, 0);
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) sum[j] = 0.f;
+                        for (int s2 = 0; s2 < k_splits; s2 += 2) {
+                            if (s2 + 1 < k_splits) ld_part(tb, s2 + 1);
+#pragma unroll
+                            for (int j = 0; j < 32; ++j) sum[j] += ta[j];
+                            if (s2 + 2 < k_splits) ld_part(ta, s2 + 2);
+                            if (s2 + 1 < k_splits) {
+#pragma unroll
+                                for (int j = 0; j < 32; ++j) sum[j] += tb[j];
                             }
-                            asm volatile("bar.sync 2, 128;" ::: "memory");
-                            const int et = threadIdx.x;             // 0..127 within the epilogue warps
-                            const int tok = tok0 + (et >> 2);
-                            const int f0 = r * 128 + (et & 3) * 32;      // first of this thread's 32 features
-                            if ((flags & EPI_ROPE) && tok < a.n_tok) {
-                                // tile r = head r of the fused projection: [0,H) query, [H,H+Hkv) key, then value heads
-                                const int head = r, q4 = et & 3;
-                                const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + q4 * 32);
-                                bf16* op;
-                                bool store = true;
-                                if (head < a.rope_H)
-                                    op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                                else {
-                                    const int hk = (head - a.rope_H) % a.rope_Hkv;
-                                    bf16* cache = (head < a.rope_H + a.rope_Hkv) ? a.k_cache : a.v_cache;
-                                    const int slot = *a.rope_pos;
-                                    // a full cache must never be written past its allocation (the host raises before launching;
-                                    // this guards graph replays whose position lives on the device)
-                                    store = slot >= 0 && slot < a.rope_Tmax;
-                                    op = cache + ((static_cast<size_t>(tok) * a.rope_Hkv + hk) * a.rope_Tmax + (store ? slot : 0)) * 128 + q4 * 32;
+                        }
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(sum[j]);
+                        if (threadIdx.x == 0) a.counters[tile] = 0;
+                    }
+                }
+                const int tok0 = c * BN;
+                if (!(flags & EPI_F32OUT) && (a.ldo & 7) == 0 && (!(flags & EPI_RESID) || ((a.ld_res & 7) == 0 && a.res_period == 0))) {
+                    // ---- transposed epilogue: this thread owns feature `feat` for 32 tokens, but the output (and the
+                    // residual) are token-major.  Pre-residual values go through a [32 tok][128 feat] bf16 smem tile so
+                    // that global traffic is 16-byte vectors along the feature dimension (4 loads + 4 stores per thread
+                    // instead of 32 + 32 scalar ones whose latencies ptxas otherwise serialises).
+                    bf16* tile = reinterpret_cast<bf16*>(epi_stage);
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) {
+                        float y;
+                        if constexpr (NA == 2)
+                            y = epi_swiglu(__uint_as_float(v[j]), __uint_as_float(u[j]));
+                        else
+                            y = epi_elem(__uint_as_float(v[j]), flags & ~EPI_RESID, bias, 0.f);
+                        tile[j * 128 + row_in_tile] = __float2bfloat16_rn(y);
+                    }
+                    asm volatile("bar.sync 2, 128;" ::: "memory");
+                    const int et = threadIdx.x;             // 0..127 within the epilogue warps
+                    const int tok = tok0 + (et >> 2);
+                    const int f0 = r * 128 + (et & 3) * 32;      // first of this thread's 32 features
+                    if ((flags & EPI_ROPE) && tok < a.n_tok) {
+                        // tile r = head r of the fused projection: [0,H) query, [H,H+Hkv) key, then value heads
+                        const int head = r, q4 = et & 3;
+                        const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + q4 * 32);
+                        bf16* op;
+                        bool store = true;
+                        if (head < a.rope_H)
+                            op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
+                        else {
+                            const int hk = (head - a.rope_H) % a.rope_Hkv;
+                            bf16* cache = (head < a.rope_H + a.rope_Hkv) ? a.k_cache : a.v_cache;
+                            const int slot = *a.rope_pos;
+                            // a full cache must never be written past its allocation (the host raises before launching;
+                            // this guards graph replays whose position lives on the device)
+                            store = slot >= 0 && slot < a.rope_Tmax;
+                            op = cache + ((static_cast<size_t>(tok) * a.rope_Hkv + hk) * a.rope_Tmax + (store ? slot : 0)) * 128 + q4 * 32;
+                        }
+                        if (!store) {
+                        } else if (head < a.rope_H + a.rope_Hkv) {
+                            const uint4* pp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + (q4 ^ 2) * 32);  // d +- 64
+                            const float2* cs = a.rope_cs + static_cast<size_t>(tok) * 64 + (q4 & 1) * 32;
+                            const float sgn = (q4 < 2) ? -1.f : 1.f;  // rotate_half: -x[d+64] for d < 64, +x[d-64] otherwise
+#pragma unroll
+                            for (int g4 = 0; g4 < 4; ++g4) {
+                                const uint4 xv = tp[g4], pv = pp[g4];
+                                const __nv_bfloat162* xh = reinterpret_cast<const __nv_bfloat162*>(&xv);
+                                const __nv_bfloat162* ph = reinterpret_cast<const __nv_bfloat162*>(&pv);
+                                uint32_t o4[4];
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const float2 xf = __bfloat1622float2(xh[e]), pf = __bfloat1622float2(ph[e]);
+                                    const float2 c0 = __ldg(cs + g4 * 8 + 2 * e), c1 = __ldg(cs + g4 * 8 + 2 * e + 1);
+                                    const float o0 = bf16_round(xf.x * c0.x) + bf16_round(sgn * pf.x * c0.y);
+                                    const float o1 = bf16_round(xf.y * c1.x) + bf16_round(sgn * pf.y * c1.y);
+                                    o4[e] = pack_bf16x2(o0, o1);
                                 }
-                                if (!store) {
-                                } else if (head < a.rope_H + a.rope_Hkv) {
-                                    const uint4* pp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + (q4 ^ 2) * 32);  // d +- 64
-                                    const float2* cs = a.rope_cs + static_cast<size_t>(tok) * 64 + (q4 & 1) * 32;
-                                    const float sgn = (q4 < 2) ? -1.f : 1.f;  // rotate_half: -x[d+64] for d < 64, +x[d-64] otherwise
+                                reinterpret_cast<uint4*>(op)[g4] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
+                            }
+                        } else {
 #pragma unroll
-                                    for (int g4 = 0; g4 < 4; ++g4) {
-                                        const uint4 xv = tp[g4], pv = pp[g4];
-                                        const __nv_bfloat162* xh = reinterpret_cast<const __nv_bfloat162*>(&xv);
-                                        const __nv_bfloat162* ph = reinterpret_cast<const __nv_bfloat162*>(&pv);
-                                        uint32_t o4[4];
+                            for (int g4 = 0; g4 < 4; ++g4) reinterpret_cast<uint4*>(op)[g4] = tp[g4];
+                        }
+                    } else if (!(flags & EPI_ROPE) && tok < a.n_tok) {
+                        const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + (et & 3) * 32);
+                        bf16* op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
+                        uint4 rv[4];
+                        if (flags & EPI_RESID) {
+                            if constexpr (NA == 1) {
+                                if (rv_ok) {   // requested before the accumulator wait (same token / features)
 #pragma unroll
-                                        for (int e = 0; e < 4; ++e) {
-                                            const float2 xf = __bfloat1622float2(xh[e]), pf = __bfloat1622float2(ph[e]);
-                                            const float2 c0 = __ldg(cs + g4 * 8 + 2 * e), c1 = __ldg(cs + g4 * 8 + 2 * e + 1);
-                                            const float o0 = bf16_round(xf.x * c0.x) + bf16_round(sgn * pf.x * c0.y);
-                                            const float o1 = bf16_round(xf.y * c1.x) + bf16_round(sgn * pf.y * c1.y);
-                                            o4[e] = pack_bf16x2(o0, o1);
-                                        }
-                                        reinterpret_cast<uint4*>(op)[g4] = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int g4 = 0; g4 < 4; ++g4) reinterpret_cast<uint4*>(op)[g4] = tp[g4];
+                                    for (int g4 = 0; g4 < 4; ++g4) rv[g4] = rv_pre[g4];
                                 }
-                            } else if (!(flags & EPI_ROPE) && tok < a.n_tok) {
-                                const uint4* tp = reinterpret_cast<const uint4*>(tile + (et >> 2) * 128 + (et & 3) * 32);
-                                bf16* op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
-                                uint4 rv[4];
+                            } else {
+                                const uint4* rp = reinterpret_cast<const uint4*>(a.resid + static_cast<size_t>(tok) * a.ld_res + f0);
+#pragma unroll
+                                for (int g4 = 0; g4 < 4; ++g4)
+                                    if (f0 + g4 * 8 < a.n_feat) rv[g4] = __ldcg(rp + g4);
+                            }
+                        }
+#pragma unroll
+                        for (int g4 = 0; g4 < 4; ++g4) {
+                            if (f0 + g4 * 8 < a.n_feat) {   // n_feat is a multiple of 8 on this path (ldo % 8 == 0)
+                                uint4 yv = tp[g4];
                                 if (flags & EPI_RESID) {
-                                    if constexpr (NA == 1) {
-                                        if (rv_ok) {   // requested before the accumulator wait (same token / features: ch == 0 for BN = 32)
+                                    const __nv_bfloat162* yh = reinterpret_cast<const __nv_bfloat162*>(&yv);
+                                    const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv[g4]);
+                                    uint32_t o4[4];
 #pragma unroll
-                                            for (int g4 = 0; g4 < 4; ++g4) rv[g4] = rv_pre[g4];
-                                        }
-                                    } else {
-                                        const uint4* rp = reinterpret_cast<const uint4*>(a.resid + static_cast<size_t>(tok) * a.ld_res + f0);
-#pragma unroll
-                                        for (int g4 = 0; g4 < 4; ++g4)
-                                            if (f0 + g4 * 8 < a.n_feat) rv[g4] = __ldcg(rp + g4);
+                                    for (int e = 0; e < 4; ++e) {
+                                        const float2 yf = __bfloat1622float2(yh[e]), rf = __bfloat1622float2(rh[e]);
+                                        o4[e] = pack_bf16x2(yf.x + rf.x, yf.y + rf.y);
                                     }
+                                    yv = make_uint4(o4[0], o4[1], o4[2], o4[3]);
                                 }
-#pragma unroll
-                                for (int g4 = 0; g4 < 4; ++g4) {
-                                    if (f0 + g4 * 8 < a.n_feat) {   // n_feat is a multiple of 8 on this path (ldo % 8 == 0)
-                                        uint4 yv = tp[g4];
-                                        if (flags & EPI_RESID) {
-                                            const __nv_bfloat162* yh = reinterpret_cast<const __nv_bfloat162*>(&yv);
-                                            const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv[g4]);
-                                            uint32_t o4[4];
-#pragma unroll
-                                            for (int e = 0; e < 4; ++e) {
-                                                const float2 yf = __bfloat1622float2(yh[e]), rf = __bfloat1622float2(rh[e]);
-                                                o4[e] = pack_bf16x2(yf.x + rf.x, yf.y + rf.y);
-                                            }
-                                            yv = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-                                        }
-                                        reinterpret_cast<uint4*>(op)[g4] = yv;
-                                    }
-                                }
+                                reinterpret_cast<uint4*>(op)[g4] = yv;
                             }
-                            asm volatile("bar.sync 2, 128;" ::: "memory");  // tile may be rewritten by the next work item
-                            continue;
                         }
                     }
-                    if (feat_ok) {
-                        float res[32];
+                    asm volatile("bar.sync 2, 128;" ::: "memory");  // tile may be rewritten by the next work item
+                    continue;
+                }
+                if (feat_ok) {
+                    float res[32];
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int tok = tok0 + j;
-                            res[j] = 0.f;
-                            if (NA == 1 && (flags & EPI_RESID) && tok < a.n_tok) {
-                                const int rr = (a.res_period > 0) ? (tok % a.res_period) : tok;
-                                res[j] = __bfloat162float(__ldcg(a.resid + static_cast<size_t>(rr) * a.ld_res + feat));
-                            }
+                    for (int j = 0; j < 32; ++j) {
+                        const int tok = tok0 + j;
+                        res[j] = 0.f;
+                        if (NA == 1 && (flags & EPI_RESID) && tok < a.n_tok) {
+                            const int rr = (a.res_period > 0) ? (tok % a.res_period) : tok;
+                            res[j] = __bfloat162float(__ldcg(a.resid + static_cast<size_t>(rr) * a.ld_res + feat));
                         }
+                    }
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int tok = tok0 + j;
-                            if (tok < a.n_tok) {
-                                float x;
-                                if constexpr (NA == 2)
-                                    x = epi_swiglu(__uint_as_float(v[j]), __uint_as_float(u[j]));
-                                else
-                                    x = epi_elem(__uint_as_float(v[j]), flags, bias, res[j]);
-                                if (flags & EPI_F32OUT)
-                                    reinterpret_cast<float*>(a.out)[static_cast<size_t>(tok) * a.ldo + feat] = x;
-                                else
-                                    reinterpret_cast<bf16*>(a.out)[static_cast<size_t>(tok) * a.ldo + feat] = __float2bfloat16_rn(x);
-                            }
+                    for (int j = 0; j < 32; ++j) {
+                        const int tok = tok0 + j;
+                        if (tok < a.n_tok) {
+                            float x;
+                            if constexpr (NA == 2)
+                                x = epi_swiglu(__uint_as_float(v[j]), __uint_as_float(u[j]));
+                            else
+                                x = epi_elem(__uint_as_float(v[j]), flags, bias, res[j]);
+                            if (flags & EPI_F32OUT)
+                                reinterpret_cast<float*>(a.out)[static_cast<size_t>(tok) * a.ldo + feat] = x;
+                            else
+                                reinterpret_cast<bf16*>(a.out)[static_cast<size_t>(tok) * a.ldo + feat] = __float2bfloat16_rn(x);
                         }
                     }
                 }
@@ -1010,86 +985,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
-template <int EPI>
-static int launch_tok(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
-                      const GemmArgs& a, cudaStream_t stream) {
-    using Cfg = TokCfg<TOK_STAGES>;
-    auto kern = gemm_tok_kernel<TOK_STAGES, EPI>;
+// One persistent CTA per SM, fewer when there are fewer work items (tiles x K splits).  The shared-memory opt-in is per
+// kernel instantiation and per device, hence one DeviceOnce per kernel.
+template <auto kern, int SMEM_BYTES, int THREADS, class... Maps>
+static int launch_gemm(const GemmArgs& a, cudaStream_t stream, const Maps&... maps) {
     static DeviceOnce once;
     if (once.first()) {
-        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     }
-    const int tiles = a.num_r_tiles * a.num_c_tiles;
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(TOK_THREADS), Cfg::SMEM_BYTES, stream, mx, mw, mo, mres, a));
+    const int items = a.num_r_tiles * a.num_c_tiles * a.k_splits;
+    const int grid = items < sm_count() ? items : sm_count();
+    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(THREADS), SMEM_BYTES, stream, maps..., a));
     return 0;
 }
-
-template <int BN, int NA, int STAGES, int EPI>
-static int launch_epi(const CUtensorMap& mr, const CUtensorMap& mc, const GemmArgs& a, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, NA, STAGES>;
-    auto kern = gemm_kernel<BN, NA, STAGES, EPI>;
-    static DeviceOnce once;
-    if (once.first()) {
-        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    }
-    const int tiles = a.num_r_tiles * a.num_c_tiles * (a.k_splits > 1 ? a.k_splits : 1);
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, mr, mc, a));
-    return 0;
-}
-
-template <int EPI>
-static int launch_wide(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
-                       const GemmArgs& a, cudaStream_t stream) {
-    using Cfg = WideCfg<WIDE_STAGES>;
-    auto kern = gemm_tok_wide_kernel<WIDE_STAGES, EPI>;
-    static DeviceOnce once;
-    if (once.first()) {
-        AF3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    }
-    const int tiles = a.num_r_tiles * a.num_c_tiles;
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    AF3_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(TOK_THREADS), Cfg::SMEM_BYTES, stream, mx, mw, mo, mres, a));
-    return 0;
-}
-
-// compile-time epilogue specialisations for the flag sets the AF3 path uses; anything else -> generic (-1, 128 x 128 tiles)
-#define AF3_TOK_EPIS(X) X(0) X(EPI_BIAS) X(EPI_BIAS | EPI_GELU) X(EPI_BIAS | EPI_RESID) X(EPI_RESID) X(EPI_SWIGLU) \
-    X(EPI_BIAS | EPI_GELU | EPI_RESID)
-static bool tok_epi_specialised(int flags) {
-#define AF3_EPI_CASE(F) case (F):
-    switch (flags) {
-        AF3_TOK_EPIS(AF3_EPI_CASE)
-        return true;
-        default:
-            return false;
-    }
-#undef AF3_EPI_CASE
-}
-
-static int launch_normal(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mo, const CUtensorMap& mres,
-                         const GemmArgs& a, bool wide, cudaStream_t stream) {
-#define AF3_EPI_CASE(F) \
-    case (F):           \
-        return wide ? launch_wide<(F)>(mx, mw, mo, mres, a, stream) : launch_tok<(F)>(mx, mw, mo, mres, a, stream);
-    if (a.tma_epi) {
-        switch (a.flags) {
-            AF3_TOK_EPIS(AF3_EPI_CASE)
-            default:
-                break;
-        }
-    }
-#undef AF3_EPI_CASE
-    return launch_tok<-1>(mx, mw, mo, mres, a, stream);
-}
-#undef AF3_TOK_EPIS
 
 template <int BN, int NA, int STAGES>
 static int launch_swap(const CUtensorMap& mr, const CUtensorMap& mc, const GemmArgs& a, cudaStream_t stream) {
 #define AF3_EPI_CASE(F) \
     case (F):           \
-        return launch_epi<BN, NA, STAGES, (F)>(mr, mc, a, stream);
+        return launch_gemm<gemm_kernel<BN, NA, STAGES, (F)>, GemmCfg<BN, NA, STAGES>::SMEM_BYTES, GEMM_THREADS>(a, stream, mr, mc);
     switch (a.flags) {
         AF3_EPI_CASE(0)
         AF3_EPI_CASE(EPI_BIAS)
@@ -1104,7 +1018,7 @@ static int launch_swap(const CUtensorMap& mr, const CUtensorMap& mc, const GemmA
             break;
     }
 #undef AF3_EPI_CASE
-    return launch_epi<BN, NA, STAGES, -1>(mr, mc, a, stream);
+    return launch_gemm<gemm_kernel<BN, NA, STAGES, -1>, GemmCfg<BN, NA, STAGES>::SMEM_BYTES, GEMM_THREADS>(a, stream, mr, mc);
 }
 
 size_t gemm_workspace_bytes() { return (8u << 20) + 4096 * sizeof(int); }
@@ -1152,11 +1066,7 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
     CUtensorMap mx, mw, mo, mres;
     const bool swap = n_tok <= 64;
     if (!swap) {
-        constexpr int BN = 128;
-        a.R = n_tok;
-        a.C = w_rows;
         a.num_r_tiles = ceil_div(n_tok, 128);
-        a.num_c_tiles = ceil_div(w_rows, BN);
         // rasterisation: GROUP_R row tiles stay L2-resident (~20 MB of the 50 MB L2) while the col-operand tiles stream
         // past them, so the streamed operand is re-read num_r_tiles / GROUP_R times instead of once per row tile
         {
@@ -1164,37 +1074,59 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
             long long g = (20ll << 20) / tile_bytes;
             a.group_r = static_cast<int>(g < 8 ? 8 : (g > 256 ? 256 : g));
         }
-        if (int e = make_tmap_2d(&mx, x, K, n_tok, ldx, BK, 128)) return e;
-        if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, swiglu ? 64 : BN)) return e;
         // smem-staged TMA-store epilogue whenever the output (and residual) layout allows 16-byte-aligned rows
         const bool res_plain = (flags & EPI_RESID) && res_period == 0;
         a.tma_epi = !(flags & EPI_F32OUT) && (ldo % 8 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
                     (!res_plain || ((ld_res % 8 == 0) && ((reinterpret_cast<uintptr_t>(resid) & 15) == 0)));
-        mo = mx;
-        mres = mx;
+        auto launch = [&](auto epi) {
+            constexpr int EPI = decltype(epi)::value;
+            // 128 x 256 tiles where the main loop is long enough to pay for an epilogue that no main loop hides.  On an H100
+            // 80GB HBM3 (700 W) they ran every K >= 3584 GEMM of config 2 7-15 % faster than the ping-pong kernel, but conv2
+            // (K = 3840, periodic residual read from global memory in the epilogue) 8 % slower, and lost up to 10 % at K = 1280
+            // (profiles/microbench_prefill_gemm.py)
+            const bool wide = EPI >= 0 && K >= 2048 && res_period == 0;
+            a.num_c_tiles = ceil_div(w_rows, wide ? 256 : 128);
+            if (int e = make_tmap_2d(&mx, x, K, n_tok, ldx, BK, 128)) return e;
+            // weight box: a 128-row half of a wide tile, a 128 x 128 tile, or the 64 gate / 64 up rows of a SwiGLU tile
+            if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, (swiglu && !wide) ? 64 : 128)) return e;
+            mo = mx;
+            mres = mx;
+            if (a.tma_epi) {
+                // [rows x 64 columns] slabs of a consumer warpgroup: one TMA store (residual: load) per 64 output columns
+                const int slab_rows = wide ? 64 : 128;
+                if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, slab_rows)) return e;
+                if (res_plain)
+                    if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, slab_rows)) return e;
+            }
+            if constexpr (EPI >= 0)
+                if (wide)
+                    return launch_gemm<gemm_tok_wide_kernel<WIDE_STAGES, EPI>, WideCfg<WIDE_STAGES>::SMEM_BYTES, TOK_THREADS>(
+                        a, stream, mx, mw, mo, mres);
+            return launch_gemm<gemm_tok_kernel<TOK_STAGES, EPI>, TokCfg<TOK_STAGES>::SMEM_BYTES, TOK_THREADS>(a, stream, mx, mw,
+                                                                                                              mo, mres);
+        };
+        // compile-time epilogues for the flag sets the AF3 path uses, only with the TMA-store epilogue; anything else runs the
+        // generic instantiation (128 x 128 tiles)
         if (a.tma_epi) {
-            // [128 rows x 64 columns] slabs: one TMA store (residual: load) per 64 output columns of a tile
-            if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 128)) return e;
-            if (res_plain)
-                if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 128)) return e;
+            switch (flags) {
+#define AF3_EPI_CASE(F) \
+    case (F):           \
+        return launch(IntC<(F)>{});
+                AF3_EPI_CASE(0)
+                AF3_EPI_CASE(EPI_BIAS)
+                AF3_EPI_CASE(EPI_BIAS | EPI_GELU)
+                AF3_EPI_CASE(EPI_BIAS | EPI_RESID)
+                AF3_EPI_CASE(EPI_RESID)
+                AF3_EPI_CASE(EPI_SWIGLU)
+                AF3_EPI_CASE(EPI_BIAS | EPI_GELU | EPI_RESID)
+#undef AF3_EPI_CASE
+                default:
+                    break;
+            }
         }
-        // 128 x 256 tiles where the main loop is long enough to pay for an epilogue that no main loop hides.  On an H100
-        // 80GB HBM3 (700 W) they ran every K >= 3584 GEMM of config 2 7-15 % faster than the ping-pong kernel, but conv2
-        // (K = 3840, periodic residual read from global memory in the epilogue) 8 % slower, and lost up to 10 % at K = 1280
-        // (profiles/microbench_prefill_gemm.py)
-        const bool wide = a.tma_epi && tok_epi_specialised(flags) && K >= 2048 && res_period == 0;
-        if (wide) {
-            a.num_c_tiles = ceil_div(w_rows, 256);
-            if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, 128)) return e;
-            if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 64)) return e;
-            if (res_plain)
-                if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 64)) return e;
-        }
-        return launch_normal(mx, mw, mo, mres, a, wide, stream);
+        return launch(IntC<-1>{});
     }
     constexpr int BN = 32;
-    a.R = w_rows;
-    a.C = n_tok;
     a.num_c_tiles = ceil_div(n_tok, BN);
     a.group_r = 1;
     if (int e = make_tmap_2d(&mw, w, K, w_rows, ldw, BK, 128)) return e;
