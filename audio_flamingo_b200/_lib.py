@@ -45,6 +45,9 @@ SIGNATURES = {
     "af3_argmax_scratch_bytes": (_sz, [_i]),
     "af3_argmax": (_i, [_p, _p, _i, _i, _p, _p]),
     "af3_token_step": (_i, [_p, _p, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
+    "af3_quant_fp8": (_i, [_p, _p, _i, _p, _p, _i, _i]),
+    "af3_gemm_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _sz]),
+    "af3_gemm_qkv_rope_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz]),
 }
 
 

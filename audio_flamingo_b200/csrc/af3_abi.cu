@@ -43,6 +43,7 @@ using af3::bf16;
 #define S(stream) reinterpret_cast<cudaStream_t>(stream)
 #define B16(p) reinterpret_cast<const bf16*>(p)
 #define B16M(p) reinterpret_cast<bf16*>(p)
+#define AF3_EPI_ROPE_INTERNAL 32  // af3::EPI_ROPE: set only by the fused q/k/v entry points
 
 extern "C" {
 
@@ -90,6 +91,30 @@ int af3_gemm_qkv_rope(void* stream, const void* x, int ldx, const void* w, int l
     af3::RopeEpilogue r{rope_cs, B16M(k_cache), B16M(v_cache), pos_dev, H, Hkv, Tmax};
     return af3::gemm_bf16(S(stream), B16(x), ldx, B16(w), ldw, q_out, ldo, n_tok, (H + 2 * Hkv) * D, K,
                           AF3_EPI_BIAS | 32, B16(bias), nullptr, 0, 0, workspace, workspace_bytes, &r);
+}
+
+int af3_quant_fp8(void* stream, const void* x, int ldx, void* q, float* scales, int rows, int K) {
+    return af3::quant_fp8(S(stream), B16(x), ldx, reinterpret_cast<uint8_t*>(q), scales, rows, K);
+}
+
+int af3_gemm_fp8(void* stream, const void* x, int ldx, const float* x_scales, const void* w, int ldw, const float* w_scale_inv,
+                 void* out, int ldo, int n_tok, int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res,
+                 void* workspace, size_t workspace_bytes) {
+    if (flags & AF3_EPI_ROPE_INTERNAL) return af3::fail("af3_gemm_fp8: use af3_gemm_qkv_rope_fp8 for the RoPE epilogue");
+    return af3::gemm_fp8(S(stream), reinterpret_cast<const uint8_t*>(x), ldx, x_scales, reinterpret_cast<const uint8_t*>(w), ldw,
+                         w_scale_inv, out, ldo, n_tok, n_feat, K, flags, B16(bias), B16(resid), ld_res, workspace, workspace_bytes,
+                         nullptr);
+}
+
+int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_scales, const void* w, int ldw,
+                          const float* w_scale_inv, const void* bias, void* q_out, int ldo, int n_tok, int K, int H, int Hkv, int D,
+                          const float* rope_cs, void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace,
+                          size_t workspace_bytes) {
+    if (D != 128) return af3::fail("af3_gemm_qkv_rope_fp8: head_dim must be 128");
+    af3::RopeEpilogue r{rope_cs, B16M(k_cache), B16M(v_cache), pos_dev, H, Hkv, Tmax};
+    return af3::gemm_fp8(S(stream), reinterpret_cast<const uint8_t*>(x), ldx, x_scales, reinterpret_cast<const uint8_t*>(w), ldw,
+                         w_scale_inv, q_out, ldo, n_tok, (H + 2 * Hkv) * D, K, AF3_EPI_BIAS | AF3_EPI_ROPE_INTERNAL, B16(bias), nullptr,
+                         0, workspace, workspace_bytes, &r);
 }
 
 int af3_pack_gate_up(void* stream, const void* gate, const void* up, void* packed, int F, int K) {

@@ -30,11 +30,11 @@ static PFN_encodeTiled get_encode() {
 }
 
 static int encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                  const cuuint32_t* box) {
+                  const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
     PFN_encodeTiled fn = get_encode();
     if (!fn) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_b,
+    CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_b,
                     box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -53,6 +53,16 @@ int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t cols, uint64_t row
     cuuint64_t strides[1] = {pitch_elems * 2};
     cuuint32_t box[2] = {box_cols, box_rows};
     return encode(map, base, 2, dims, strides, box);
+}
+
+int make_tmap_2d_u8(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch_bytes, uint32_t box_cols,
+                    uint32_t box_rows) {
+    if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("TMA base pointer must be 16-byte aligned");
+    if (pitch_bytes % 16 != 0) return fail("TMA row pitch must be a multiple of 16 bytes");
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {pitch_bytes};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    return encode(map, base, 2, dims, strides, box, CU_TENSOR_MAP_DATA_TYPE_UINT8);
 }
 
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t p1_elems,

@@ -1,9 +1,12 @@
 // HBM-bound CUDA-core kernels of the AF3 path: LayerNorm, AvgPool+LayerNorm, RMSNorm, conv-stem im2col,
-// rotary embedding + KV-cache append, embedding gather / audio-row scatter, gate/up weight packing, argmax.
+// rotary embedding + KV-cache append, embedding gather / audio-row scatter, gate/up weight packing, argmax, FP8 activation
+// quantization.
 // All bf16 tensors are accessed with 16-byte vector loads/stores, one warp (or a few) per row, fp32 statistics,
 // and the reference's bf16 rounding points are reproduced op by op (cited per kernel).
 #include "common.h"
 #include "ptx.cuh"
+
+#include <cuda_fp8.h>
 
 namespace af3 {
 
@@ -26,6 +29,63 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 }
 
 constexpr int NORM_MAXV = 16;  // uint4 chunks per lane -> dim <= 4096
+
+// ---------------------------------------------------------------------------------------------------------
+// FP8 activation quantization (include/af3b200.h af3_quant_fp8), the input side of the FP8 decoder projections that
+// replaces the activation quantization of [O] integrations/finegrained_fp8.py FP8Linear.forward.  Per row and 128-column
+// group: amax = max |x| (fp32, exact from bf16), s = amax / 448 rounded to nearest (s = 1 for an all-zero group),
+// q = e4m3(x / s) rounded to nearest even with saturation -- torch's (x.float() / s).to(torch.float8_e4m3fn) bit for bit.
+// One warp per row and pair of groups: each half-warp owns one group, 16-byte loads (8 bf16) and 8-byte stores per lane.
+// q: [rows][K] e4m3 (pitch K); scales: [K / 128][rows] fp32, so that a GEMM's k-block reads the scales of consecutive
+// tokens from consecutive addresses.
+__global__ void __launch_bounds__(256)
+quant_fp8_kernel(const bf16* __restrict__ x, int ldx, uint8_t* __restrict__ q, float* __restrict__ scales, int rows, int K,
+                 unsigned long long* trace) {
+    if (threadIdx.x == 0) trace_mark(trace, 0);
+    pdl_launch_dependents();
+    pdl_wait();
+    if (threadIdx.x == 0) trace_mark(trace, 1);
+    const int pairs = (K + 255) >> 8;
+    const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (w < rows * pairs) {  // warp-uniform: every lane takes part in the shuffles
+        const int row = w / pairs;
+        const int col = ((w - row * pairs) << 8) + lane * 8;
+        const bool ok = col < K;
+        float f[8];
+        unpack8(ok ? __ldcs(reinterpret_cast<const uint4*>(x + static_cast<size_t>(row) * ldx + col)) : make_uint4(0, 0, 0, 0), f);
+        float amax = 0.f;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) amax = fmaxf(amax, fabsf(f[e]));
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));  // within the half-warp
+        const float s = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+        uint32_t packed[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(f[4 * h], s), __fdiv_rn(f[4 * h + 1], s)),
+                                                                     __NV_SATFINITE, __NV_E4M3);
+            const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(f[4 * h + 2], s), __fdiv_rn(f[4 * h + 3], s)),
+                                                                     __NV_SATFINITE, __NV_E4M3);
+            packed[h] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+        }
+        if (ok) {
+            *reinterpret_cast<uint2*>(q + static_cast<size_t>(row) * K + col) = make_uint2(packed[0], packed[1]);
+            if ((lane & 15) == 0) scales[static_cast<size_t>(col >> 7) * rows + row] = s;
+        }
+    }
+    if (threadIdx.x == 0) trace_mark(trace, 3);
+}
+
+int quant_fp8(cudaStream_t stream, const bf16* x, int ldx, uint8_t* q, float* scales, int rows, int K) {
+    AF3_REQUIRE(rows > 0 && K > 0 && K % 128 == 0, "quant_fp8: K must be a positive multiple of 128");
+    AF3_REQUIRE(ldx >= K && ldx % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 7) == 0,
+                "quant_fp8: x must be 16-byte aligned with a pitch that is a multiple of 8 elements, q 8-byte aligned");
+    const long long warps = static_cast<long long>(rows) * ((K + 255) / 256);
+    AF3_CHECK_CUDA(launch_kernel(quant_fp8_kernel, dim3(static_cast<unsigned>((warps + 7) / 8)), dim3(256), 0, stream, x, ldx, q, scales,
+                                 rows, K, trace_next_slot()));
+    return 0;
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // LayerNorm ([O] AF3M:224,232,366: nn.LayerNorm, eps 1e-5; fp32 statistics, one rounding to bf16).

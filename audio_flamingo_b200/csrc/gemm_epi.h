@@ -21,5 +21,11 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
               int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, int res_period,
               void* workspace, size_t workspace_bytes, const RopeEpilogue* rope);
 size_t gemm_workspace_bytes();
+// Block-scaled FP8 GEMM (include/af3b200.h af3_gemm_fp8): x e4m3 [n_tok, K] (pitch ldx bytes) with group scales
+// sx [K/128][n_tok], w e4m3 [rows, K] (pitch ldw bytes) with weight_scale_inv sw [rows/128][K/128]
+int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, const uint8_t* w, int ldw, const float* sw,
+             void* out, int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res,
+             void* workspace, size_t workspace_bytes, const RopeEpilogue* rope);
+int quant_fp8(cudaStream_t stream, const bf16* x, int ldx, uint8_t* q, float* scales, int rows, int K);
 
 }  // namespace af3

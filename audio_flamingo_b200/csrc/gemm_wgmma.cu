@@ -20,6 +20,9 @@
 //                  reference's bf16 rounding points -> stmatrix into a 128B-swizzled bf16 slab -> TMA store.  While
 //                  one warpgroup runs its epilogue the other runs its main loop, so the tensor cores stay busy.
 //
+// gemm_fp8_tok_kernel (FP8 normal mode, n_tok > 64): the wide kernel's layout with e4m3 operands and 128 x 128 tiles; each
+//                  k-block is promoted out of the QGMMA accumulator with its block scales (see the kernel).
+//
 // gemm_kernel (few-token / swap mode, decode), 9 warps:
 //   warp 8         TMA producer, as above.
 //   warps 0-7      two consumer warpgroups: wgmma.mma_async (m64 x BN x 16) straight from the ring, each warpgroup
@@ -27,6 +30,8 @@
 //                  from which warps 0-3 (one row per lane) run the epilogue and the split-K reduction.
 //   "Row operand" = the matrix whose rows are the wgmma M dimension (128 per tile) = weight features (so every wgmma
 //   streams weight rows), "col operand" = the tokens (BN = 32); the epilogue writes the transposed tile.
+//   With FP8 = true (gemm_fp8, n_tok <= 64) both operands are block-scaled e4m3 and each 128-wide k-block is
+//   promoted out of the QGMMA accumulator into fp32 with its scales.
 //
 // Shared pieces, written once: the ring cursor (Ring), the consumer k-loop of all three kernels (ring_mma / ring_drain),
 // and for the two token-major kernels the shared-memory carve-up and prologue (TokSmem, tok_prologue), the producer loop
@@ -75,6 +80,10 @@ struct GemmArgs {
     float* ws;      // [tiles][k_splits][BN][128] fp32
     int* counters;  // [tiles], zero on entry, reset to zero by the reducing CTA
     unsigned long long* trace;  // in-graph timeline slot of this launch (common.h) or nullptr
+    // FP8 few-token kernel: activation group scales sx [K/128][n_tok], weight_scale_inv sw [w_rows/128][ld_sw]
+    const float* sx;
+    const float* sw;
+    int ld_sw;
 };
 
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
@@ -175,6 +184,7 @@ struct OutSlabs {
 template <int STAGES_>
 struct TokCfg {
     static constexpr int STAGES = STAGES_;
+    static constexpr int KB = BK;                        // K elements per k-block
     static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
     static constexpr int STAGE_BYTES = 2 * X_BYTES;      // + 128 weight rows x 64
     using Out = OutSlabs<128, 2>;                        // per consumer warpgroup: the 128 output columns of its tile
@@ -191,6 +201,7 @@ constexpr int TOK_STAGES = 4;
 template <int STAGES_>
 struct WideCfg {
     static constexpr int STAGES = STAGES_;
+    static constexpr int KB = BK;
     static constexpr int X_BYTES = 128 * BK * 2;         // 128 token rows x 64
     static constexpr int W_BYTES = 256 * BK * 2;         // 256 weight rows x 64
     static constexpr int STAGE_BYTES = X_BYTES + W_BYTES;
@@ -204,6 +215,21 @@ struct WideCfg {
 // the staging (two epilogue passes) was as fast within run-to-run spread (prefill GEMMs -1.5 to +5 %, their time-weighted
 // sum 0.5 % slower) and needs the second pass.
 constexpr int WIDE_STAGES = 3;
+
+// FP8 token-major tiles: 128 tokens x 128 weight rows, one k-block = 128 e4m3 = one 128-byte swizzle row = one scale group
+template <int STAGES_>
+struct Fp8TokCfg {
+    static constexpr int STAGES = STAGES_;
+    static constexpr int KB = 128;
+    static constexpr int X_BYTES = 128 * 128;            // 128 token rows x 128 e4m3
+    static constexpr int STAGE_BYTES = 2 * X_BYTES;      // + 128 weight rows x 128 e4m3
+    using Out = OutSlabs<64, 2>;                         // per consumer warpgroup: its 64 x 128 half of the output tile
+    static constexpr int STAGING_BYTES = 2 * Out::BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert((2 * STAGES + 4) * 8 <= 256, "barrier area");
+    static_assert(SMEM_BYTES <= 232448, "shared memory per CTA");
+};
+constexpr int FP8_TOK_STAGES = 6;
 
 // ---- few-token (swap) mode
 constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma; warps 0-3 also run the epilogue), warp 8: TMA producer
@@ -322,7 +348,7 @@ __device__ __forceinline__ void tok_prologue(const TokSmem<Cfg>& sm, uint32_t em
 template <class Cfg, class LoadW>
 __device__ __forceinline__ void tok_produce(const TokSmem<Cfg>& sm, const CUtensorMap* map_x, const GemmArgs& a, LoadW&& load_w) {
     const int num_tiles = a.num_r_tiles * a.num_c_tiles;
-    const int kb_n = (a.K + BK - 1) / BK;
+    const int kb_n = (a.K + Cfg::KB - 1) / Cfg::KB;
     Ring<Cfg::STAGES> ring;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int r, c;
@@ -332,8 +358,8 @@ __device__ __forceinline__ void tok_produce(const TokSmem<Cfg>& sm, const CUtens
             uint64_t* bar = &sm.full[ring.stage];
             mbar_wait(&sm.empty[ring.stage], ring.phase ^ 1);
             mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
-            tma_load_2d(sX, map_x, bar, kb * BK, r * 128);
-            load_w(sX + Cfg::X_BYTES, bar, kb * BK, c);
+            tma_load_2d(sX, map_x, bar, kb * Cfg::KB, r * 128);
+            load_w(sX + Cfg::X_BYTES, bar, kb * Cfg::KB, c);
             ring.next();
         }
     }
@@ -644,13 +670,123 @@ gemm_tok_wide_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
+// ============================================================================ normal mode, FP8 (gemm_fp8, n_tok > 64)
+// One 128 (tokens) x 128 (weight rows) tile per CTA at a time, both operands block-scaled e4m3.  Consumer warpgroup cw owns
+// token rows [64 cw, 64 cw + 64) and all 128 columns: four m64n128k32 QGMMAs per k-block into a k-block accumulator (64
+// fp32), which is then promoted into the main accumulator (64 fp32) with sx of the thread's two token rows times sw of the
+// column's 128-row weight block.  A 128 x 128 tile per warpgroup would need 256 accumulator registers per thread.  The weight
+// rows of a tile are two 64-row halves: rows [128 c, 128 c + 128), or with SwiGLU the 64 gate rows 64 c.. and the 64 up rows
+// of the same features of the [gate; up] layout, which lie in different scale blocks -- hence one scale per column half.
+// The epilogue rounds the result to bf16 (FP8Linear's output) and then runs the bf16 kernels' register epilogue.
+template <int STAGES, int EPI>
+__global__ void __launch_bounds__(TOK_THREADS, 1)
+gemm_fp8_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+                    const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const GemmArgs a) {
+    static_assert(EPI >= 0 && !(EPI & (EPI_F32OUT | EPI_GELU | EPI_ROPE)), "FP8 epilogues: bias, residual, SwiGLU");
+    using Cfg = Fp8TokCfg<STAGES>;
+    extern __shared__ uint8_t smem_raw[];
+    const TokSmem<Cfg> sm(smem_raw);
+
+    const int wg = threadIdx.x >> 7;
+    const int tw = threadIdx.x & 127;
+    constexpr int flags = EPI;
+    constexpr bool swiglu = flags & EPI_SWIGLU;
+    constexpr int OUT_COLS = swiglu ? 64 : 128;
+    constexpr bool tma_res = flags & EPI_RESID;
+
+    // `empty`: 8 arrivals, one per consumer warp, since both warpgroups read every stage
+    if (threadIdx.x == 0) tok_prologue(sm, 8, false, a, &map_x, &map_w, &map_out, &map_res, true, tma_res);
+    __syncthreads();
+    pdl_launch_dependents();
+
+    // weight-row halves of column tile c
+    auto w_row = [&](int c, int h) { return swiglu ? h * a.swiglu_up_row0 + c * 64 : c * 128 + h * 64; };
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tw == 0) {
+            pdl_wait();
+            tok_produce(sm, &map_x, a, [&](uint8_t* sW, uint64_t* bar, int k0, int c) {
+                tma_load_2d(sW, &map_w, bar, k0, w_row(c, 0));
+                tma_load_2d(sW + 64 * 128, &map_w, bar, k0, w_row(c, 1));
+            });
+        }
+    } else {
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;
+        const bool leader = tw == 0;
+        const typename Cfg::Out slabs{sm.staging + cw * Cfg::Out::BYTES};
+        const int num_tiles = a.num_r_tiles * a.num_c_tiles;
+        const int kb_n = a.K / 128;
+        pdl_wait();  // activation scales, residual reads and output writes are ordered after every earlier kernel
+        if (threadIdx.x == 128) trace_mark(a.trace, 1);
+        uint32_t rpar = 0;
+        Ring<STAGES> ring;
+        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+            int r, c;
+            tile_coords(t, a, r, c);
+            const int row0 = r * 128 + cw * 64;
+            const int out_col0 = c * OUT_COLS;
+            if (tma_res && leader) slabs.load_res(&map_res, &sm.rbar[cw], out_col0, row0, a.n_feat);
+            // scale rows: sw of the two column halves, sx of this thread's two token rows (0 past n_tok)
+            const float* swp0 = a.sw + static_cast<size_t>(w_row(c, 0) / 128) * a.ld_sw;
+            const float* swp1 = a.sw + static_cast<size_t>(w_row(c, 1) / 128) * a.ld_sw;
+            const int tok0 = row0 + frag_row(tw, 0), tok1 = row0 + frag_row(tw, 2);
+            const bool ok0 = tok0 < a.n_tok, ok1 = tok1 < a.n_tok;
+
+            float acc[64], kacc[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = kacc[i] = 0.f;
+            for (int kb = 0; kb < kb_n; ++kb) {
+                const float sw0 = __ldg(swp0 + kb), sw1 = __ldg(swp1 + kb);
+                const float sx0 = ok0 ? a.sx[static_cast<size_t>(kb) * a.n_tok + tok0] : 0.f;
+                const float sx1 = ok1 ? a.sx[static_cast<size_t>(kb) * a.n_tok + tok1] : 0.f;
+                mbar_wait(&sm.full[ring.stage], ring.phase);
+                const uint32_t sX = smem_u32(sm.ring + ring.stage * Cfg::STAGE_BYTES) + cw * 64 * 128;
+                const uint32_t sW = smem_u32(sm.ring + ring.stage * Cfg::STAGE_BYTES) + Cfg::X_BYTES;
+                fence_regs(kacc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    wgmma_m64n128k32_e4m3(kacc, make_smem_desc_sw128(sX + k * 32, 0, 1024), make_smem_desc_sw128(sW + k * 32, 0, 1024), k > 0);
+                wgmma_commit();
+                wgmma_wait<0>();  // the k-block's partial sums are final: promote them
+                fence_regs(kacc);
+                if ((tw & 31) == 0) mbar_arrive(&sm.empty[ring.stage]);
+                ring.next();
+                const float s00 = sx0 * sw0, s01 = sx0 * sw1, s10 = sx1 * sw0, s11 = sx1 * sw1;
+#pragma unroll
+                for (int i = 0; i < 64; ++i) {
+                    // register i: row +8 when (i >> 1) & 1, column 8 (i >> 2) + ...: the upper column half from i = 32 on
+                    const float sc = ((i >> 1) & 1) ? (i < 32 ? s10 : s11) : (i < 32 ? s00 : s01);
+                    acc[i] = fmaf(kacc[i], sc, acc[i]);
+                }
+            }
+            if (threadIdx.x == 128) trace_mark(a.trace, 2);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = bf16_round(acc[i]);  // FP8Linear returns its matmul in bf16
+
+            slabs.acquire(leader, tma_res, 1 + cw, &sm.rbar[cw], rpar);
+            epi_fragment<128, tma_res ? 1 : 0>(acc, slabs, 0, row0, out_col0, flags, a);
+            slabs.store(leader, 1 + cw, &map_out, OUT_COLS / 64, out_col0, row0, a.n_feat);
+        }
+        if (leader) bulk_wait_read<0>();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) trace_mark(a.trace, 3);
+}
+
 // ============================================================================ few-token (swap) mode (n_tok <= 64)
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches, full ILP across the 32-column chunk);
 // EPI < 0: generic instantiation reading a.flags at run time (odd layouts / unusual flag mixes).
-template <int BN, int NA, int STAGES, int EPI>
+// FP8: both operands e4m3 with block scales (gemm_fp8).  A stage then holds 128 K (one 128-byte swizzle row = one scale
+// group) in the same bytes as 64 bf16 K.  Each k-block is accumulated by m64n32k32 QGMMAs into its own registers and
+// promoted into the fp32 accumulator with sw (of the weight rows' 128-row block) x sx (of each token column), so the
+// tensor-core accumulation never spans two k-blocks.  The epilogue first rounds the result to bf16 (FP8Linear's output).
+template <int BN, int NA, int STAGES, int EPI, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_c, const GemmArgs a) {
     using Cfg = GemmCfg<BN, NA, STAGES>;
+    constexpr int KB = FP8 ? 128 : BK;  // K elements per k-block (128 bytes of every row either way)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     float* accbuf = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
@@ -678,11 +814,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 
     const int k_splits = a.k_splits;
     const int num_tiles = a.num_r_tiles * a.num_c_tiles * k_splits;  // work items: (tile, split), split fastest
-    const int k_blocks_total = (a.K + BK - 1) / BK;
+    const int k_blocks_total = (a.K + KB - 1) / KB;
     // K range of split s: blocks [kb_lo(s), kb_lo(s+1)), sizes differ by at most one
     auto kb_lo = [&](int s) { return (s * k_blocks_total) / k_splits; };
 
     if (warp == 8) {
+        if constexpr (FP8) {
+            // the weight scales of the first work item, like its weights, do not depend on earlier kernels: into L2 now
+            if (blockIdx.x < num_tiles) {
+                int r, c;
+                tile_coords(blockIdx.x / k_splits, a, r, c);
+#pragma unroll
+                for (int na = 0; na < NA; ++na) {
+                    const float* row = a.sw + static_cast<size_t>(a.swiglu_up_row0 ? (na * a.swiglu_up_row0) / 128 + r : r * NA + na) * a.ld_sw;
+                    for (int j = lane * 32; j < a.ld_sw; j += 32 * 32) prefetch_l2(row + j);
+                }
+            }
+        }
         if (lane == 0) {
             Ring<STAGES> ring;
             // The row operand is a WEIGHT matrix, independent of earlier kernels -> its first STAGES tiles are
@@ -699,7 +847,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         uint8_t* sR = smem + prefetched * Cfg::STAGE_BYTES;
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
-                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[prefetched], kb * BK,
+                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[prefetched], kb * KB,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
                 }
@@ -718,10 +866,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         mbar_arrive_expect_tx(&full[ring.stage], Cfg::STAGE_BYTES);
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
-                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[ring.stage], kb * BK,
+                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[ring.stage], kb * KB,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
-                    tma_load_2d(sC, &map_c, &full[ring.stage], kb * BK, c * BN);
+                    tma_load_2d(sC, &map_c, &full[ring.stage], kb * KB, c * BN);
                     ring.next();
                 }
             }
@@ -750,20 +898,81 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 #pragma unroll
                     for (int na = 0; na < NA; ++na) fence_regs(accr[na]);
                 };
-                const int held = ring_mma(ring, full, empty, kb_lo(sp + 1) - kb_lo(sp), [&](int stage) {
-                    const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t sC = sR + Cfg::R_BYTES;
+                if constexpr (FP8) {
+                    int r, c;
+                    tile_coords(t / k_splits, a, r, c);
+                    // sw rows of the NA 128-row weight blocks; sx of this thread's 8 token columns (frag_col), 0 past n_tok
+                    const float* swp[NA];
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t bdesc = make_smem_desc_sw128(sC + k * 32, 0, 1024);
+                    for (int na = 0; na < NA; ++na)
+                        swp[na] = a.sw + static_cast<size_t>(a.swiglu_up_row0 ? (na * a.swiglu_up_row0) / 128 + r : r * NA + na) * a.ld_sw;
+                    const float* sxp[8];
+                    bool sx_ok[8];
 #pragma unroll
-                        for (int na = 0; na < NA; ++na) {
-                            const uint64_t adesc = make_smem_desc_sw128(sR + na * 128 * BK * 2 + wg * 64 * 128 + k * 32, 0, 1024);
-                            wgmma_m64n32_ss<0, 0>(accr[na], adesc, bdesc, 1);
-                        }
+                    for (int j = 0; j < 8; ++j) {
+                        const int tok = c * BN + frag_col(tw, 2 * (j >> 1) * 2 + (j & 1));
+                        sx_ok[j] = tok < a.n_tok;
+                        sxp[j] = a.sx + (sx_ok[j] ? tok : 0);
                     }
-                }, fence);
-                ring_drain(empty, held, fence);
+                    float kacc[NA][BN / 2];
+#pragma unroll
+                    for (int na = 0; na < NA; ++na)
+#pragma unroll
+                        for (int i = 0; i < BN / 2; ++i) kacc[na][i] = 0.f;
+                    const bool lane0 = lane == 0;
+                    for (int kb = kb_lo(sp); kb < kb_lo(sp + 1); ++kb) {
+                        // scales first: their loads are in flight while the stage lands
+                        float sw[NA], sx[8];
+#pragma unroll
+                        for (int na = 0; na < NA; ++na) sw[na] = __ldg(swp[na] + kb);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) sx[j] = sx_ok[j] ? sxp[j][static_cast<size_t>(kb) * a.n_tok] : 0.f;
+                        mbar_wait(&full[ring.stage], ring.phase);
+                        const uint32_t sR = smem_u32(smem + ring.stage * Cfg::STAGE_BYTES);
+                        const uint32_t sC = sR + Cfg::R_BYTES;
+#pragma unroll
+                        for (int na = 0; na < NA; ++na) fence_regs(kacc[na]);
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            const uint64_t bdesc = make_smem_desc_sw128(sC + k * 32, 0, 1024);
+#pragma unroll
+                            for (int na = 0; na < NA; ++na) {
+                                const uint64_t adesc = make_smem_desc_sw128(sR + na * 128 * BK * 2 + wg * 64 * 128 + k * 32, 0, 1024);
+                                wgmma_m64n32k32_e4m3(kacc[na], adesc, bdesc, k > 0);
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();  // the k-block's partial sums are final: promote them
+#pragma unroll
+                        for (int na = 0; na < NA; ++na) fence_regs(kacc[na]);
+                        if (lane0) mbar_arrive(&empty[ring.stage]);
+                        ring.next();
+#pragma unroll
+                        for (int na = 0; na < NA; ++na)
+#pragma unroll
+                            for (int i = 0; i < BN / 2; ++i) {
+                                // register i holds column frag_col(tw, i): column pair (i >> 2, i & 1) of this thread
+                                const int j = 2 * (i >> 2) + (i & 1);
+                                accr[na][i] = fmaf(kacc[na][i], sw[na] * sx[j], accr[na][i]);
+                            }
+                    }
+                } else {
+                    const int held = ring_mma(ring, full, empty, kb_lo(sp + 1) - kb_lo(sp), [&](int stage) {
+                        const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+                        const uint32_t sC = sR + Cfg::R_BYTES;
+#pragma unroll
+                        for (int k = 0; k < BK / 16; ++k) {
+                            const uint64_t bdesc = make_smem_desc_sw128(sC + k * 32, 0, 1024);
+#pragma unroll
+                            for (int na = 0; na < NA; ++na) {
+                                const uint64_t adesc = make_smem_desc_sw128(sR + na * 128 * BK * 2 + wg * 64 * 128 + k * 32, 0, 1024);
+                                wgmma_m64n32_ss<0, 0>(accr[na], adesc, bdesc, 1);
+                            }
+                        }
+                    }, fence);
+                    ring_drain(empty, held, fence);
+                }
                 asm volatile("bar.sync 3, 256;" ::: "memory");  // the previous tile's epilogue is done with accbuf
 #pragma unroll
                 for (int na = 0; na < NA; ++na)
@@ -847,6 +1056,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
 #pragma unroll
                         for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(sum[j]);
                         if (threadIdx.x == 0) a.counters[tile] = 0;
+                    }
+                }
+                if constexpr (FP8) {  // FP8Linear returns its matmul in bf16; bias / residual / SwiGLU act on that
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) {
+                        v[j] = __float_as_uint(bf16_round(__uint_as_float(v[j])));
+                        if constexpr (NA == 2) u[j] = __float_as_uint(bf16_round(__uint_as_float(u[j])));
                     }
                 }
                 const int tok0 = c * BN;
@@ -1023,6 +1239,25 @@ static int launch_swap(const CUtensorMap& mr, const CUtensorMap& mc, const GemmA
 
 size_t gemm_workspace_bytes() { return (8u << 20) + 4096 * sizeof(int); }
 
+// split-K of the few-token mode: when the tile grid cannot fill the GPU and a (zero-initialised) workspace was supplied,
+// split the kb_total k-blocks of every tile over s CTAs
+static void choose_k_splits(GemmArgs& a, int kb_total, void* workspace, size_t workspace_bytes) {
+    a.k_splits = 1;
+    const int tiles = a.num_r_tiles * a.num_c_tiles;
+    if (workspace && workspace_bytes >= gemm_workspace_bytes() && tiles * 2 <= sm_count() && tiles <= 4096) {
+        int s = sm_count() / tiles;
+        const int forced = [] { const char* e = getenv("AF3_KSPLIT"); return e ? atoi(e) : 0; }();  // experiments only (read per call)
+        if (forced > 0) s = forced;
+        if (s > kb_total / 4) s = kb_total / 4;  // keep at least 4 k-blocks per split
+        if (s > 16) s = 16;
+        if (s >= 2 && static_cast<size_t>(tiles) * s * 32 * 128 * sizeof(float) <= (8u << 20)) {
+            a.k_splits = s;
+            a.ws = reinterpret_cast<float*>(workspace);
+            a.counters = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(workspace) + (8u << 20));
+        }
+    }
+}
+
 // Host entry.  x: [n_tok, K] bf16 (pitch ldx), w: [n_rows_w, K] bf16 (pitch ldw) where n_rows_w = n_feat, or the
 // gate/up-interleaved 2*ceil(n_feat/128)*128 rows when EPI_SWIGLU.  out: [n_tok, n_feat] (pitch ldo).
 int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, void* out, int ldo, int n_tok,
@@ -1138,24 +1373,110 @@ int gemm_bf16(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ld
         return launch_swap<BN, 2, 5>(mw, mx, a, stream);
     }
     a.num_r_tiles = ceil_div(w_rows, 128);
-    // split-K when the tile grid cannot fill the GPU and a (zero-initialised) workspace was supplied
-    a.k_splits = 1;
-    const int tiles = a.num_r_tiles * a.num_c_tiles;
-    const int kb_total = ceil_div(K, BK);
-    if (workspace && workspace_bytes >= gemm_workspace_bytes() && tiles * 2 <= sm_count() && tiles <= 4096) {
-        int s = sm_count() / tiles;
-        const int forced = [] { const char* e = getenv("AF3_KSPLIT"); return e ? atoi(e) : 0; }();  // experiments only (read per call)
-        if (forced > 0) s = forced;
-        if (s > kb_total / 4) s = kb_total / 4;  // keep at least 4 k-blocks per split
-        if (s > 16) s = 16;
-        if (s >= 2 && static_cast<size_t>(tiles) * s * BN * 128 * sizeof(float) <= (8u << 20)) {
-            a.k_splits = s;
-            a.ws = reinterpret_cast<float*>(workspace);
-            a.counters = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(workspace) + (8u << 20));
-        }
-    }
+    choose_k_splits(a, ceil_div(K, BK), workspace, workspace_bytes);
     // ring depth: 10 x 20 KB = 200 KB in flight per SM (the few-token streams are latency-bound on bytes in flight)
     return launch_swap<BN, 1, 10>(mw, mx, a, stream);
+}
+
+// Host entry of the block-scaled FP8 GEMM (include/af3b200.h af3_gemm_fp8): up to 64 tokens the few-token kernel with e4m3
+// operands (split-K, RoPE epilogue), above that gemm_fp8_tok_kernel.  Epilogues: none, bias, residual, SwiGLU on [gate; up],
+// bias + RoPE + KV append (few-token only).
+int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, const uint8_t* w, int ldw, const float* sw,
+             void* out, int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res,
+             void* workspace, size_t workspace_bytes, const RopeEpilogue* rope) {
+    AF3_REQUIRE(n_tok > 0 && n_feat > 0 && K > 0, "gemm_fp8: empty problem");
+    AF3_REQUIRE(K % 128 == 0 && n_feat % 128 == 0, "gemm_fp8: K and n_feat must be multiples of 128 (the scale blocks)");
+    AF3_REQUIRE(ldx % 16 == 0 && ldw % 16 == 0 && ldx >= K && ldw >= K, "gemm_fp8: pitches must be multiples of 16 bytes");
+    AF3_REQUIRE(sx && sw, "gemm_fp8: scale pointers required");
+    AF3_REQUIRE(!(flags & EPI_BIAS) || bias, "gemm_fp8: bias flag without pointer");
+    AF3_REQUIRE(!(flags & EPI_RESID) || resid, "gemm_fp8: residual flag without pointer");
+    const bool swiglu = flags & EPI_SWIGLU;
+    AF3_REQUIRE(!swiglu || (flags & EPI_SWIGLU_CONCAT), "gemm_fp8: SwiGLU needs the [gate; up] layout (AF3_EPI_SWIGLU_CONCAT)");
+    flags &= ~EPI_SWIGLU_CONCAT;
+    const bool rope_epi = flags & EPI_ROPE;
+    AF3_REQUIRE(flags == 0 || flags == EPI_BIAS || flags == EPI_RESID || flags == EPI_SWIGLU || flags == (EPI_BIAS | EPI_ROPE),
+                "gemm_fp8: supported epilogues are none, bias, residual, SwiGLU and bias + RoPE");
+    AF3_REQUIRE((ldo % 8) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "gemm_fp8: out must be 16-byte aligned, ldo % 8 == 0");
+    AF3_REQUIRE(!(flags & EPI_RESID) || ((ld_res % 8) == 0 && (reinterpret_cast<uintptr_t>(resid) & 15) == 0),
+                "gemm_fp8: resid must be 16-byte aligned, ld_res % 8 == 0");
+    const int w_rows = swiglu ? 2 * n_feat : n_feat;
+    GemmArgs a{};
+    a.K = K;
+    a.n_tok = n_tok;
+    a.n_feat = n_feat;
+    a.out = out;
+    a.ldo = ldo;
+    a.bias = bias;
+    a.resid = resid;
+    a.ld_res = ld_res;
+    a.flags = flags;
+    a.swiglu_up_row0 = swiglu ? n_feat : 0;
+    a.sx = sx;
+    a.sw = sw;
+    a.ld_sw = K / 128;
+    a.k_splits = 1;
+    a.trace = trace_next_slot();
+    if (rope_epi) {
+        AF3_REQUIRE(rope && rope->cs && rope->k_cache && rope->v_cache && rope->pos, "gemm_fp8: EPI_ROPE needs the rope arguments");
+        AF3_REQUIRE(n_tok <= 64 && n_feat == (rope->H + 2 * rope->Hkv) * 128, "gemm_fp8: EPI_ROPE is the few-token fused q/k/v projection with head_dim 128");
+        a.rope_cs = reinterpret_cast<const float2*>(rope->cs);
+        a.k_cache = rope->k_cache;
+        a.v_cache = rope->v_cache;
+        a.rope_pos = rope->pos;
+        a.rope_H = rope->H;
+        a.rope_Hkv = rope->Hkv;
+        a.rope_Tmax = rope->Tmax;
+    }
+    if (n_tok > 64) {
+        // token-major tiles: rows = tokens, cols = 128 weight rows (64 outputs with SwiGLU)
+        a.num_r_tiles = ceil_div(n_tok, 128);
+        a.num_c_tiles = w_rows / 128;
+        {  // as gemm_bf16: GROUP_R token tiles (~20 MB) stay L2-resident while the weight tiles stream past them
+            const long long g = (20ll << 20) / (128ll * K);
+            a.group_r = static_cast<int>(g < 8 ? 8 : (g > 256 ? 256 : g));
+        }
+        CUtensorMap mx, mw, mo, mres;
+        if (int e = make_tmap_2d_u8(&mx, x, K, n_tok, ldx, 128, 128)) return e;
+        if (int e = make_tmap_2d_u8(&mw, w, K, w_rows, ldw, 128, 64)) return e;
+        if (int e = make_tmap_2d(&mo, out, n_feat, n_tok, ldo, 64, 64)) return e;
+        mres = mo;
+        if (flags & EPI_RESID)
+            if (int e = make_tmap_2d(&mres, resid, n_feat, n_tok, ld_res, 64, 64)) return e;
+        switch (flags) {
+#define AF3_EPI_CASE(F) \
+    case (F):           \
+        return launch_gemm<gemm_fp8_tok_kernel<FP8_TOK_STAGES, (F)>, Fp8TokCfg<FP8_TOK_STAGES>::SMEM_BYTES, TOK_THREADS>(a, stream, mx, mw, mo, mres);
+            AF3_EPI_CASE(0)
+            AF3_EPI_CASE(EPI_BIAS)
+            AF3_EPI_CASE(EPI_RESID)
+            AF3_EPI_CASE(EPI_SWIGLU)
+#undef AF3_EPI_CASE
+            default:
+                return fail("gemm_fp8: unsupported epilogue");
+        }
+    }
+    constexpr int BN = 32;
+    a.num_c_tiles = ceil_div(n_tok, BN);
+    a.num_r_tiles = ceil_div(w_rows, swiglu ? 256 : 128);
+    a.group_r = 1;
+    CUtensorMap mw, mx;
+    if (int e = make_tmap_2d_u8(&mw, w, K, w_rows, ldw, 128, 128)) return e;
+    if (int e = make_tmap_2d_u8(&mx, x, K, n_tok, ldx, 128, BN)) return e;
+    if (swiglu)  // ring depth as in gemm_bf16: as many stages as fit beside the accumulator tile
+        return launch_gemm<gemm_kernel<BN, 2, 5, EPI_SWIGLU, true>, GemmCfg<BN, 2, 5>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
+    choose_k_splits(a, K / 128, workspace, workspace_bytes);
+    switch (flags) {
+#define AF3_EPI_CASE(F) \
+    case (F):           \
+        return launch_gemm<gemm_kernel<BN, 1, 10, (F), true>, GemmCfg<BN, 1, 10>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
+        AF3_EPI_CASE(0)
+        AF3_EPI_CASE(EPI_BIAS)
+        AF3_EPI_CASE(EPI_RESID)
+        AF3_EPI_CASE(EPI_BIAS | EPI_ROPE)
+#undef AF3_EPI_CASE
+        default:
+            return fail("gemm_fp8: unsupported epilogue");
+    }
 }
 
 }  // namespace af3

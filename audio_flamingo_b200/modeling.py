@@ -66,6 +66,37 @@ def _cfg_get(cfg, name, default=None):
 
 
 # =====================================================================================================
+# FP8 weights (FineGrainedFP8 layout, [O] integrations/finegrained_fp8.py:793-905, weight_block_size = (128, 128))
+# =====================================================================================================
+FP8_MAX = 448.0
+DECODER_PROJECTIONS = ("self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "mlp.gate_proj",
+                       "mlp.up_proj", "mlp.down_proj")
+
+
+def quantize_fp8_blocks(w):
+    """Fp8Quantize.convert with 128 x 128 blocks: per-block amax, scale = 448 / amax in fp32 (1 for an all-zero block),
+    q = e4m3(clamp(w * scale)), weight_scale_inv = 1 / scale.  w [rows, cols], both multiples of 128 -> (q, weight_scale_inv
+    fp32 [rows / 128, cols / 128]).  Load-time only; runs wherever w lives."""
+    rows, cols = w.shape
+    blocks = w.to(torch.float32).reshape(rows // 128, 128, cols // 128, 128)
+    amax = blocks.abs().amax(dim=(1, 3))
+    scale = torch.where(amax > 0, FP8_MAX / torch.where(amax > 0, amax, torch.ones_like(amax)), torch.ones_like(amax))
+    q = torch.clamp(blocks * scale[:, None, :, None], min=-FP8_MAX, max=FP8_MAX).to(torch.float8_e4m3fn)
+    return q.reshape(rows, cols), (1.0 / scale).to(torch.float32)
+
+
+def dequantize_fp8_blocks(q, scale_inv):
+    """Fp8Dequantize: q [rows, cols] e4m3 times its block's weight_scale_inv, in fp32."""
+    rows, cols = q.shape
+    return (q.to(torch.float32).reshape(rows // 128, 128, cols // 128, 128) * scale_inv[:, None, :, None]).reshape(rows, cols)
+
+
+def _is_decoder_projection(key):
+    """'language_model.model.layers.<i>.<proj>' for the seven FP8 projections of a decoder layer"""
+    return key.startswith("language_model.model.layers.") and any(key.endswith("." + p) for p in DECODER_PROJECTIONS)
+
+
+# =====================================================================================================
 # parameter holders (names == reference state_dict keys)
 # =====================================================================================================
 class _EncAttn(nn.Module):
@@ -285,6 +316,54 @@ class AF3KVCache:
         self.k, self.v, self.Tmax = k, v, new_T
 
 
+class _Bf16Projections:
+    """The four GEMMs of one decoder layer on bf16 weights (chosen once, at pack time)."""
+
+    def __init__(self, lm, wqkv, bqkv, wo, wgu, wdown):
+        self.lm, self.wqkv, self.bqkv, self.wo, self.wgu, self.wdown = lm, wqkv, bqkv, wo, wgu, wdown
+
+    def qkv(self, y):
+        return ops.linear(y, self.wqkv, self.bqkv)
+
+    def qkv_rope(self, y, kc, vc, rope_cs, pos_dev):
+        lm = self.lm
+        return ops.qkv_rope_linear(y, self.wqkv, self.bqkv, kc, vc, H=lm.H, Hkv=lm.Hkv, D=lm.D, rope_cs=rope_cs, pos_dev=pos_dev)
+
+    def o(self, a, h):
+        ops.linear(a, self.wo, resid=h, out=h)
+
+    def gate_up(self, y):
+        return ops.swiglu_linear(y, self.wgu, self.lm.inter, concat=self.lm._swiglu_concat)
+
+    def down(self, g, h):
+        ops.linear(g, self.wdown, resid=h, out=h)
+
+
+class _Fp8Projections:
+    """The same four GEMMs on block-scaled e4m3 weights: every input is quantized (af3_quant_fp8) right before its GEMM.
+    Each weight is a (e4m3 matrix, weight_scale_inv) pair."""
+
+    def __init__(self, lm, wqkv, bqkv, wo, wgu, wdown):
+        self.lm, self.wqkv, self.bqkv, self.wo, self.wgu, self.wdown = lm, wqkv, bqkv, wo, wgu, wdown
+
+    def qkv(self, y):
+        return ops.linear_fp8(ops.quant_fp8(y), *self.wqkv, self.bqkv)
+
+    def qkv_rope(self, y, kc, vc, rope_cs, pos_dev):
+        lm = self.lm
+        return ops.qkv_rope_linear_fp8(ops.quant_fp8(y), *self.wqkv, self.bqkv, kc, vc, H=lm.H, Hkv=lm.Hkv, D=lm.D, rope_cs=rope_cs,
+                                       pos_dev=pos_dev)
+
+    def o(self, a, h):
+        ops.linear_fp8(ops.quant_fp8(a), *self.wo, resid=h, out=h)
+
+    def gate_up(self, y):
+        return ops.swiglu_linear_fp8(ops.quant_fp8(y), *self.wgu, self.lm.inter)
+
+    def down(self, g, h):
+        ops.linear_fp8(ops.quant_fp8(g), *self.wdown, resid=h, out=h)
+
+
 class Qwen2ForCausalLM(nn.Module):
     """Decoder ([O] Q2M:332-487) on sm_90a kernels: RMSNorm, fused QKV GEMM (+bias), RoPE + in-place KV append,
     wgmma causal GQA attention (prefill) / split-KV decode attention, o GEMM (+residual), fused SwiGLU GEMM,
@@ -306,7 +385,9 @@ class Qwen2ForCausalLM(nn.Module):
             raise AF3Error("only default RoPE is implemented")
         self.model = _Qwen2Model(tc)
         self.lm_head = nn.Linear(self.hid, self.vocab, bias=False)
+        self.quantization = None  # "fp8": the decoder projections hold e4m3 weights + weight_scale_inv (load_reference_state_dict)
         self._packed = None
+        self._proj = None
         self._inv_freq = None
 
     def pack_weights(self):
@@ -318,6 +399,8 @@ class Qwen2ForCausalLM(nn.Module):
         P = []
         HD, KD = self.H * self.D, self.Hkv * self.D
         self._swiglu_concat = self.inter % 128 == 0
+        if self.quantization == "fp8":
+            return self._pack_fp8()
         for l in self.model.layers:
             a, m = l.self_attn, l.mlp
             wqkv = torch.cat([a.q_proj.weight.detach(), a.k_proj.weight.detach(), a.v_proj.weight.detach()], 0).contiguous()
@@ -331,6 +414,34 @@ class Qwen2ForCausalLM(nn.Module):
                 wgu = ops.pack_gate_up(m.gate_proj.weight.detach().contiguous(), m.up_proj.weight.detach().contiguous())
             P.append((wqkv, bqkv, wgu))
         self._packed = P
+        self._proj = [_Bf16Projections(self, wqkv, bqkv, l.self_attn.o_proj.weight, wgu, l.mlp.down_proj.weight)
+                      for l, (wqkv, bqkv, wgu) in zip(self.model.layers, P)]
+        self._set_inv_freq()
+
+    def _pack_fp8(self):
+        """FP8 counterpart of pack_weights: one fused [q; k; v] and one [gate; up] e4m3 matrix per layer, each with its fused
+        weight_scale_inv grid; the projections' weight / weight_scale_inv are re-pointed at row views of them."""
+        P, proj = [], []
+        HD, KD = self.H * self.D, self.Hkv * self.D
+        for l in self.model.layers:
+            a, m = l.self_attn, l.mlp
+            wqkv = torch.cat([a.q_proj.weight.detach(), a.k_proj.weight.detach(), a.v_proj.weight.detach()], 0).contiguous()
+            sqkv = torch.cat([a.q_proj.weight_scale_inv, a.k_proj.weight_scale_inv, a.v_proj.weight_scale_inv], 0).contiguous()
+            bqkv = torch.cat([a.q_proj.bias.detach(), a.k_proj.bias.detach(), a.v_proj.bias.detach()], 0).contiguous()
+            wgu = torch.cat([m.gate_proj.weight.detach(), m.up_proj.weight.detach()], 0).contiguous()
+            sgu = torch.cat([m.gate_proj.weight_scale_inv, m.up_proj.weight_scale_inv], 0).contiguous()
+            for mod, w, sc, r0, r1 in ((a.q_proj, wqkv, sqkv, 0, HD), (a.k_proj, wqkv, sqkv, HD, HD + KD), (a.v_proj, wqkv, sqkv, HD + KD, HD + 2 * KD),
+                                       (m.gate_proj, wgu, sgu, 0, self.inter), (m.up_proj, wgu, sgu, self.inter, 2 * self.inter)):
+                mod.weight.data = w[r0:r1]
+                mod.weight_scale_inv = sc[r0 // 128:r1 // 128]
+            a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data = bqkv[:HD], bqkv[HD:HD + KD], bqkv[HD + KD:]
+            P.append((wqkv, bqkv, wgu))
+            proj.append(_Fp8Projections(self, (wqkv, sqkv), bqkv, (a.o_proj.weight, a.o_proj.weight_scale_inv), (wgu, sgu),
+                                        (m.down_proj.weight, m.down_proj.weight_scale_inv)))
+        self._packed, self._proj = P, proj
+        self._set_inv_freq()
+
+    def _set_inv_freq(self):
         # Qwen2RotaryEmbedding.compute_default_rope_parameters, evaluated on the CPU like the reference (Q2M:86-89)
         inv = 1.0 / (self.rope_theta ** (torch.arange(0, self.D, 2, dtype=torch.int64).to(dtype=torch.float) / self.D))
         self._inv_freq = inv.to(self.lm_head.weight.device)
@@ -356,35 +467,34 @@ class Qwen2ForCausalLM(nn.Module):
         if fused_qkv:
             rope_cs = ops.rope_table(B, D, cache.pos_dev, cache.kv_start, self._inv_freq)
         y = None
-        for li, (l, (wqkv, bqkv, wgu)) in enumerate(zip(self.model.layers, self._packed)):
+        for li, (l, pj) in enumerate(zip(self.model.layers, self._proj)):
             kc, vc = cache.k[li], cache.v[li]
             a = torch.empty((B * T, H * D), device=h.device, dtype=bf16)
             if decode:
                 if fused_qkv:
                     # q/k/v projection with RoPE + KV append in the GEMM epilogue (rope table: once per step, above)
                     y = ops.rmsnorm(h, l.input_layernorm.weight, self.eps, out=y)
-                    qkv = ops.qkv_rope_linear(y, wqkv, bqkv, kc, vc, H=H, Hkv=Hkv, D=D, rope_cs=rope_cs, pos_dev=cache.pos_dev)
+                    qkv = pj.qkv_rope(y, kc, vc, rope_cs, cache.pos_dev)
                 else:
                     # more than 64 sequences per GPU: token-major tensor-core GEMM + the stand-alone RoPE / append kernel reading
                     # the slot from device memory (graph replay)
                     y = ops.rmsnorm(h, l.input_layernorm.weight, self.eps, out=y)
-                    qkv = ops.linear(y, wqkv, bqkv)
+                    qkv = pj.qkv(y)
                     ops.rope_kv_append(qkv, kc, vc, B=B, T=1, H=H, Hkv=Hkv, D=D, pos0=0, inv_freq=self._inv_freq,
                                        kv_start=cache.kv_start, pos0_dev=cache.pos_dev)
                 ops.decode_attention(qkv, kc, vc, a, scratch, B=B, H=H, Hkv=Hkv, D=D, ctx_len=cache.ctx_dev,
                                      kv_start=cache.kv_start, scale=D ** -0.5)
             else:
                 y = ops.rmsnorm(h, l.input_layernorm.weight, self.eps, out=y)
-                qkv = ops.linear(y, wqkv, bqkv)
+                qkv = pj.qkv(y)
                 ops.rope_kv_append(qkv, kc, vc, B=B, T=T, H=H, Hkv=Hkv, D=D, pos0=pos0, inv_freq=self._inv_freq,
                                    kv_start=cache.kv_start)
                 ops.attention(qkv, kc, vc, a.view(B, T, H * D), B=B, H=H, Hkv=Hkv, D=D, Tq=T, Tk=pos0 + T, scale=D ** -0.5,
                               causal=True, kv_layout=1, Tk_pitch=cache.Tmax, ldq=(H + 2 * Hkv) * D, ldk=D,
                               kv_start=cache.kv_start)
-            ops.linear(a, l.self_attn.o_proj.weight, resid=h, out=h)
+            pj.o(a, h)
             y = ops.rmsnorm(h, l.post_attention_layernorm.weight, self.eps, out=y)
-            g = ops.swiglu_linear(y, wgu, self.inter, concat=self._swiglu_concat)
-            ops.linear(g, l.mlp.down_proj.weight, resid=h, out=h)
+            pj.down(pj.gate_up(y), h)
         return h
 
     def _head(self, h, row_idx=None):
@@ -471,24 +581,83 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
 
     # ---- construction from the reference model / a reference state_dict
     @classmethod
-    def from_reference(cls, ref_model, device="cuda"):
-        """Build from an instantiated reference model (weights are copied, cast to bf16)."""
+    def from_reference(cls, ref_model, device="cuda", quantization=None):
+        """Build from an instantiated reference model (weights are copied, cast to bf16).  quantization="fp8": see
+        load_reference_state_dict."""
         m = cls(ref_model.config)
-        m.load_reference_state_dict(ref_model.state_dict(), device=device)
+        m.load_reference_state_dict(ref_model.state_dict(), device=device, quantization=quantization)
         m.generation_config = getattr(ref_model, "generation_config", None)
         return m
 
-    def load_reference_state_dict(self, sd, device="cuda"):
+    @property
+    def quantization(self):
+        return self.language_model.quantization
+
+    def load_reference_state_dict(self, sd, device="cuda", quantization=None):
+        """Load a reference state_dict.  Weights are cast to bf16.
+
+        quantization="fp8" stores the seven projections of every decoder layer (q, k, v, o, gate, up, down) as block-scaled
+        e4m3 -- the FineGrainedFP8 format of transformers with 128 x 128 blocks: e4m3 weights plus one fp32 weight_scale_inv
+        per block, quantized from the bf16 values exactly as Fp8Quantize does -- and runs them on the FP8 GEMMs with
+        activations quantized per token and 128 columns.  The embedding, lm_head, audio tower and projector stay bf16.  The
+        hidden, q/k/v/o and intermediate sizes must be multiples of 128.
+
+        The state_dict may already be in that layout (`<name>.weight` float8_e4m3fn plus `<name>.weight_scale_inv`, what
+        state_dict() of an FP8 model returns).  Its decoder projections are then used as they are, and the model is FP8
+        whatever `quantization` says.  Any other Linear stored that way is dequantized once to bf16."""
+        if quantization not in (None, "fp8"):
+            raise AF3Error(f"quantization must be None or 'fp8', got {quantization!r}")
+        scaled = {k[: -len(".weight_scale_inv")] for k in sd if k.endswith(".weight_scale_inv")}
+        if any(_is_decoder_projection(k) for k in scaled):
+            quantization = "fp8"
+        lm = self.language_model
+        for name in DECODER_PROJECTIONS:  # back to the plain bf16 module tree (a previous FP8 load added the scales)
+            for l in lm.model.layers:
+                mod = l.get_submodule(name)
+                if "weight_scale_inv" in mod._buffers:
+                    del mod._buffers["weight_scale_inv"]
+        if quantization == "fp8":
+            sizes = {"hidden_size": lm.hid, "q size": lm.H * lm.D, "k/v size": lm.Hkv * lm.D, "intermediate_size": lm.inter}
+            bad = {k: v for k, v in sizes.items() if v % 128}
+            if bad:
+                raise AF3Error(f"fp8 quantization needs multiples of 128 (the 128 x 128 scale blocks); got {bad}")
         self.to_empty(device=device)
         self.to(bf16)
         own = self.state_dict()
         missing = [k for k in own if k not in sd]
-        unexpected = [k for k in sd if k not in own]
+        unexpected = [k for k in sd if k not in own and not (k.endswith(".weight_scale_inv") and k[: -len("_scale_inv")] in own)]
         if missing or unexpected:
             raise AF3Error(f"state_dict mismatch: missing {missing[:4]}..., unexpected {unexpected[:4]}...")
+
+        def bf16_value(k):
+            v = sd[k]
+            if v.dtype == torch.float8_e4m3fn:
+                base = k[: -len(".weight")]
+                if base not in scaled:
+                    raise AF3Error(f"{k} is float8_e4m3fn without {base}.weight_scale_inv")
+                dev = torch.device(device)
+                return dequantize_fp8_blocks(v.to(dev), sd[base + ".weight_scale_inv"].to(dev, torch.float32)).to(bf16)
+            return v
+
+        fp8_params = {}
         with torch.no_grad():
             for k, v in own.items():
-                v.copy_(sd[k].to(device=v.device, dtype=bf16))
+                base = k[: -len(".weight")] if k.endswith(".weight") else None
+                if quantization == "fp8" and base is not None and _is_decoder_projection(base):
+                    if sd[k].dtype == torch.float8_e4m3fn and base not in scaled:
+                        raise AF3Error(f"{k} is float8_e4m3fn without {base}.weight_scale_inv")
+                    if base in scaled and sd[k].dtype == torch.float8_e4m3fn:
+                        q, s = sd[k].to(v.device), sd[base + ".weight_scale_inv"].to(v.device, torch.float32)
+                    else:
+                        q, s = quantize_fp8_blocks(sd[k].to(device=v.device, dtype=bf16))
+                    fp8_params[base] = (q.contiguous(), s.contiguous())
+                    continue
+                v.copy_(bf16_value(k).to(device=v.device, dtype=bf16))
+            for base, (q, s) in fp8_params.items():
+                mod = self.get_submodule(base)
+                mod.weight = nn.Parameter(q, requires_grad=False)
+                mod.register_buffer("weight_scale_inv", s)
+        lm.quantization = quantization
         self.audio_tower._packed = None
         self.language_model._packed = None
         self._graph = None

@@ -139,6 +139,108 @@ def swiglu_linear(x, w_packed, n_feat, out=None, concat=False):
     return out
 
 
+# ----------------------------------------------------------------------------------------------- FP8 decoder projections
+fp8 = torch.float8_e4m3fn
+
+
+def quant_fp8(x, out=None, scales=None):
+    """Dynamic 1 x 128 activation quantization (include/af3b200.h af3_quant_fp8).  x bf16 [rows, K], unit column stride (the
+    row pitch may exceed K) -> (q float8_e4m3fn [rows, K], scales fp32 [K / 128, rows])."""
+    lib = _lib.load()
+    if not x.is_cuda or x.dtype != bf16 or x.dim() != 2 or x.stride(1) != 1:
+        raise _lib.AF3Error("quant_fp8: x must be a CUDA bf16 [rows, K] tensor with unit column stride")
+    rows, K = x.shape
+    if out is None:
+        out = torch.empty((rows, K), device=x.device, dtype=fp8)
+    if scales is None:
+        scales = torch.empty((K // 128, rows), device=x.device, dtype=torch.float32)
+    # the kernel writes q with pitch K and the scales as [K / 128][rows]: caller buffers must have exactly that layout
+    _req(out, fp8, "out"), _req(scales, torch.float32, "scales")
+    if tuple(out.shape) != (rows, K) or tuple(scales.shape) != (K // 128, rows):
+        raise _lib.AF3Error(f"quant_fp8: out must be [{rows}, {K}] and scales [{K // 128}, {rows}], got {tuple(out.shape)} and {tuple(scales.shape)}")
+    with _Timed(("quant_fp8", rows, K, 0, 0)):
+        check(lib.af3_quant_fp8(stream_ptr(), ptr(x), x.stride(0), ptr(out), ptr(scales), rows, K), "af3_quant_fp8")
+    _count(1)
+    return out, scales
+
+
+def _fp8_operands(xq, w, w_scale_inv):
+    q, sx = xq
+    _req(q, fp8, "x"), _req(sx, torch.float32, "x_scales"), _req(w, fp8, "w"), _req(w_scale_inv, torch.float32, "w_scale_inv")
+    n_tok, K = q.shape
+    if tuple(sx.shape) != (K // 128, n_tok) or tuple(w_scale_inv.shape) != (w.shape[0] // 128, K // 128) or w.shape[1] != K:
+        raise _lib.AF3Error(f"fp8 GEMM: shapes x {tuple(q.shape)}, x_scales {tuple(sx.shape)}, w {tuple(w.shape)}, "
+                            f"w_scale_inv {tuple(w_scale_inv.shape)} do not match")
+    return q, sx, n_tok, K
+
+
+def linear_fp8(xq, w, w_scale_inv, bias=None, *, resid=None, out=None):
+    """FP8Linear with 128 x 128 weight blocks: out = bf16(x @ w.T, block-scaled) [+ bias, rounded again] [+ resid].
+    xq = quant_fp8(x); w float8_e4m3fn [n_feat, K]; w_scale_inv fp32 [n_feat / 128, K / 128]."""
+    lib = _lib.load()
+    q, sx, n_tok, K = _fp8_operands(xq, w, w_scale_inv)
+    n_feat = w.shape[0]
+    flags = 0
+    if bias is not None:
+        _req(bias, bf16, "bias")
+        flags |= EPI_BIAS
+    if resid is not None:
+        _req(resid, bf16, "resid")
+        flags |= EPI_RESID
+    if out is None:
+        out = torch.empty((n_tok, n_feat), device=q.device, dtype=bf16)
+    ws = gemm_workspace(q.device) if n_tok <= 64 else None
+    with _Timed(("gemm_fp8", n_tok, n_feat, K, flags)):
+        check(
+            lib.af3_gemm_fp8(stream_ptr(), ptr(q), q.stride(0), ptr(sx), ptr(w), w.stride(0), ptr(w_scale_inv), ptr(out), out.stride(0),
+                             n_tok, n_feat, K, flags, ptr(bias), ptr(resid), resid.stride(0) if resid is not None else 0,
+                             ptr(ws), ws.numel() if ws is not None else 0),
+            "af3_gemm_fp8",
+        )
+    _count(1)
+    return out
+
+
+def swiglu_linear_fp8(xq, w_gate_up, w_scale_inv, n_feat, out=None):
+    """out = silu(bf16(x @ gate.T)) * bf16(x @ up.T) with FP8 weights: w_gate_up the [gate; up] concatenation
+    [2 n_feat, K], w_scale_inv its [2 n_feat / 128, K / 128] block scales."""
+    lib = _lib.load()
+    q, sx, n_tok, K = _fp8_operands(xq, w_gate_up, w_scale_inv)
+    if w_gate_up.shape[0] != 2 * n_feat:
+        raise _lib.AF3Error("swiglu_linear_fp8: w_gate_up must hold 2 * n_feat rows")
+    if out is None:
+        out = torch.empty((n_tok, n_feat), device=q.device, dtype=bf16)
+    with _Timed(("gemm_fp8", n_tok, n_feat, K, EPI_SWIGLU)):
+        check(
+            lib.af3_gemm_fp8(stream_ptr(), ptr(q), q.stride(0), ptr(sx), ptr(w_gate_up), w_gate_up.stride(0), ptr(w_scale_inv), ptr(out),
+                             out.stride(0), n_tok, n_feat, K, EPI_SWIGLU | EPI_SWIGLU_CONCAT, None, None, 0, None, 0),
+            "af3_gemm_fp8(swiglu)",
+        )
+    _count(1)
+    return out
+
+
+def qkv_rope_linear_fp8(xq, w, w_scale_inv, bias, k_cache, v_cache, *, H, Hkv, D, rope_cs, pos_dev, out=None):
+    """FP8 counterpart of qkv_rope_linear (few-token decode step): returns the [n_tok, (H+2Hkv)*D] buffer whose first H*D
+    columns hold the rotated queries; rotated keys and the values go straight into the caches."""
+    lib = _lib.load()
+    q, sx, n_tok, K = _fp8_operands(xq, w, w_scale_inv)
+    _req(bias, bf16, "bias")
+    if out is None:
+        out = torch.empty((n_tok, (H + 2 * Hkv) * D), device=q.device, dtype=bf16)
+    ws = gemm_workspace(q.device)
+    Tmax = k_cache.shape[2]
+    with _Timed(("gemm_fp8", n_tok, (H + 2 * Hkv) * D, K, EPI_BIAS | 32)):
+        check(
+            lib.af3_gemm_qkv_rope_fp8(stream_ptr(), ptr(q), q.stride(0), ptr(sx), ptr(w), w.stride(0), ptr(w_scale_inv), ptr(bias), ptr(out),
+                                      out.stride(0), n_tok, K, H, Hkv, D, ptr(rope_cs), ptr(k_cache), ptr(v_cache), Tmax, ptr(pos_dev),
+                                      ptr(ws), ws.numel()),
+            "af3_gemm_qkv_rope_fp8",
+        )
+    _count(1)
+    return out
+
+
 # ----------------------------------------------------------------------------------------------- log-mel
 class LogMelTables:
     """Constant tables of the log-mel kernel, built exactly as the reference builds its constants."""

@@ -5,7 +5,7 @@
  * it replaces ([O] = transformers 5.5.0, the executable statement of the AF3 path; see SURVEY.md section 0):
  *   AF3M = models/audioflamingo3/modeling_audioflamingo3.py   WFE = models/whisper/feature_extraction_whisper.py
  *   Q2M  = models/qwen2/modeling_qwen2.py                      GEN = generation/utils.py
- *   CACHE = cache_utils.py   SDPA = integrations/sdpa_attention.py
+ *   CACHE = cache_utils.py   SDPA = integrations/sdpa_attention.py   FP8 = integrations/finegrained_fp8.py
  *
  * Conventions: plain pointers and sizes only (no torch types); every pointer is a DEVICE pointer unless the
  * parameter name starts with h_; `stream` is a cudaStream_t passed as void*; all calls are asynchronous on
@@ -73,6 +73,37 @@ int af3_gemm_bf16_ws(void* stream, const void* x, int ldx, const void* w, int ld
 
 /* gate [F,K], up [F,K] -> packed [2*ceil(F/128)*128, K]: per 128 features, 128 gate rows then 128 up rows. */
 int af3_pack_gate_up(void* stream, const void* gate, const void* up, void* packed, int F, int K);
+
+/* ---- FP8 decoder projections (block-scaled e4m3, the FineGrainedFP8 format of [O] FP8:793-865 with 128 x 128 weight
+ * blocks).  ABI v4 gained these three entry points additively; nothing else changed.  Together they replace the
+ * FP8Linear.forward calls ([O] FP8:248-284): activation quantization, block-scaled matmul, bias.
+ *
+ * Activation quantization rule (per token row and 128-column group): amax = max |x| in fp32 from the bf16 values,
+ * s = amax / 448 (IEEE division, round to nearest), or s = 1 when amax == 0; q = e4m3(x / s) rounded to nearest even with
+ * saturation -- what torch's (x.float() / s).to(torch.float8_e4m3fn) gives.
+ * Scale layouts: activation scales are [K/128][rows] fp32 (group g of row t at scales[g * rows + t]); weight scales are
+ * weight_scale_inv as stored by FineGrainedFP8, [w_rows/128][K/128] fp32 row-major.
+ *
+ * x bf16 [rows, K] (pitch ldx elements, 16-byte aligned) -> q e4m3 [rows, K] (pitch K bytes), scales [K/128][rows].
+ * K % 128 == 0. */
+int af3_quant_fp8(void* stream, const void* x, int ldx, void* q, float* scales, int rows, int K);
+
+/* out[t, n] = epi( bf16( sum_kb (sum_{k in kb} x[t,k] w[n,k]) * x_scales[kb][t] * w_scale_inv[n/128][kb] ) ): each 128-wide
+ * k-block's partial sum leaves the tensor-core accumulator and is scaled in fp32.  x e4m3 [n_tok, K] (pitch ldx bytes) with
+ * x_scales from af3_quant_fp8 (n_tok rows); w e4m3 [n_feat, K] (pitch ldw bytes), or with AF3_EPI_SWIGLU |
+ * AF3_EPI_SWIGLU_CONCAT the [gate (n_feat rows); up (n_feat rows)] concatenation.  flags: 0, AF3_EPI_BIAS (bias added to
+ * the bf16 matmul result, then rounded again, as FP8Linear does), AF3_EPI_RESID (out = bf16(result + resid); out may alias
+ * resid) or AF3_EPI_SWIGLU | AF3_EPI_SWIGLU_CONCAT.  K and n_feat % 128 == 0; out / resid 16-byte aligned with pitches that
+ * are multiples of 8.  The workspace is that of af3_gemm_bf16_ws (split-K for few-token calls). */
+int af3_gemm_fp8(void* stream, const void* x, int ldx, const float* x_scales, const void* w, int ldw, const float* w_scale_inv,
+                 void* out, int ldo, int n_tok, int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res,
+                 void* workspace, size_t workspace_bytes);
+
+/* FP8 counterpart of af3_gemm_qkv_rope: same outputs and cache writes, from the quantized x and the FP8 [q; k; v] weight. */
+int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_scales, const void* w, int ldw,
+                          const float* w_scale_inv, const void* bias, void* q_out, int ldo, int n_tok, int K, int H, int Hkv, int D,
+                          const float* rope_cs, void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace,
+                          size_t workspace_bytes);
 
 /* Log-mel front end; replaces WhisperFeatureExtractor._torch_extract_fbank_features ([O] WFE:135-164).
  * wave fp32 [n_win, n_samples] (zero padded to 30 s by the caller as WFE:296 does), mel_filters fp32 [201,128]

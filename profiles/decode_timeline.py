@@ -34,6 +34,7 @@ def main():
     ap.add_argument("--prompt", type=int, default=780)
     ap.add_argument("--new-tokens", type=int, default=24)
     ap.add_argument("--layers", type=int, default=28)
+    ap.add_argument("--fp8", action="store_true", help="FP8 decoder projections (load_reference_state_dict(quantization='fp8'))")
     args = ap.parse_args()
 
     import bench
@@ -48,6 +49,8 @@ def main():
     model.to_empty(device=dev)
     model.to(torch.bfloat16)
     bench.init_synthetic_weights_(model, seed=0)
+    if args.fp8:
+        model.load_reference_state_dict(model.state_dict(), device=dev, quantization="fp8")
     rs = np.random.RandomState(0)
     ids = torch.from_numpy(rs.randint(1, 151643, size=(args.batch, args.prompt)).astype(np.int64)).to(dev)
     am = torch.ones_like(ids)
@@ -96,7 +99,9 @@ def main():
         lines.append(f"| {r['kind']} | {r['ctas']} | {f(r['entry_min'])}..{f(r['entry_max'])} | {f(r['wait_min'])}..{f(r['wait_max'])} | "
                      f"{f(r['mid_max'])} | {f(r['exit_min'])}..{f(r['exit_max'])} |")
     Path(base + ".md").write_text("\n".join(lines) + "\n")
-    print(json.dumps({k: out[k] for k in ("tag", "decode_ms_per_step_events", "step_us_from_trace", "launches_in_graph")}))
+    quant_us = sum(v["slot_us"] for k, v in agg.items() if k.startswith("quant_fp8"))
+    out["quant_fp8_share"] = quant_us / step_us
+    print(json.dumps({k: out[k] for k in ("tag", "decode_ms_per_step_events", "step_us_from_trace", "launches_in_graph", "quant_fp8_share")}))
 
 
 if __name__ == "__main__":
