@@ -190,7 +190,8 @@ int af3_embed_scatter(void* stream, const int64_t* ids, int n_tok, const void* e
                       int64_t audio_token_id, const void* audio_embeds, int n_win, int frames, const int* post_len,
                       void* out, int* scratch_rows /*[n_tok]*/, int* counts /*[2]*/);
 
-/* Greedy step (GEN:2762-2800): argmax over fp32 logits [B, V] (first max index, like torch.argmax).
+/* Greedy step (GEN:2762-2800): argmax over fp32 logits [B, V] -> the first index of the row maximum.  Unlike torch.argmax,
+ * which returns the index of a NaN, NaN entries are skipped; an all-NaN row yields 0.
  * scratch: af3_argmax_scratch_bytes(B) bytes of device memory (two-stage reduction). */
 size_t af3_argmax_scratch_bytes(int B);
 int af3_argmax(void* stream, const float* logits, int B, int V, int64_t* out_ids, void* scratch);

@@ -5,6 +5,7 @@ import math
 import numpy as np
 import pytest
 import torch
+from test_cuda_core_kernels_gpu import logmel_reference, rope_reference
 
 pytestmark = pytest.mark.gpu
 bf16 = torch.bfloat16
@@ -218,6 +219,24 @@ def _sdpa_ref(q, k, v, scale, mask):
     return p @ v
 
 
+def _peak_scores(q, k, kind, scale, first, last, j):
+    """Overwrite q (every head = e_0) and k[..., 0] so that the attention score of the key at position j is a chosen profile
+    (natural-log units): 'rising' climbs by 20 per 128 keys up to the key at `last` (the running maximum moves every chunk and
+    the online-softmax rescale is << 1), 'falling' is its mirror (maximum at `first`), 'two_peaks' has equal peaks at `first` and
+    `last` and falls by 0.3 per key between them (partials whose maxima differ by hundreds).  'random' leaves both alone."""
+    if kind == "random":
+        return
+    if kind == "rising":
+        f = 20 / 128 * (j - last)
+    elif kind == "falling":
+        f = -20 / 128 * (j - first)
+    else:
+        f = -0.3 * torch.minimum((j - first).abs(), (j - last).abs())
+    q.zero_()
+    q[..., 0] = 1.0
+    k[..., 0] = (f / scale).to(k.dtype)
+
+
 @pytest.fixture(params=["v2", "v1"])
 def attn_impl(request, monkeypatch):
     """Both row tilings of the prefill / encoder attention kernel go through the same parity cases: v2 (two consumer warpgroups,
@@ -246,12 +265,17 @@ def test_attention_bidirectional(ops, attn_impl, D, H, T, lens):
     _close(out, ref, 2e-2, 2e-2, f"attention D={D} T={T}")
 
 
-@pytest.mark.parametrize("T,starts", [(256, None), (300, [0, 37, 250]), (130, [5, 129]), (780, [0, 3, 530]), (1000, None), (64, None),
-                                      (129, [0, 128]), (513, [0, 400, 512])])
-def test_attention_causal_gqa_cache(ops, attn_impl, T, starts):
+@pytest.mark.parametrize("T,starts,scores", [(256, None, "random"), (300, [0, 37, 250], "random"), (130, [5, 129], "random"),
+                                             (780, [0, 3, 530], "random"), (1000, None, "random"), (64, None, "random"),
+                                             (129, [0, 128], "random"), (513, [0, 400, 512], "random"),
+                                             (1000, [0, 3, 530], "rising"), (1000, [0, 3, 530], "falling"), (780, None, "two_peaks")])
+def test_attention_causal_gqa_cache(ops, attn_impl, T, starts, scores):
     H, Hkv, D, Tmax = 8, 2, 128, 1024
     B = len(starts) if starts else 2
     qkv = _rand((B * T, (H + 2 * Hkv) * D), 1.0, 41)
+    tok = torch.arange(T, device="cuda", dtype=torch.float32).repeat(B)[:, None]
+    _peak_scores(qkv[:, :H * D].view(B * T, H, D), qkv[:, H * D:(H + Hkv) * D].view(B * T, Hkv, D), scores, D ** -0.5,
+                 T // 4, T - 1 if scores == "rising" else 3 * T // 4, tok)
     k_cache = torch.zeros((B, Hkv, Tmax, D), device="cuda", dtype=bf16)
     v_cache = torch.zeros_like(k_cache)
     kk = qkv[:, H * D:(H + Hkv) * D].view(B, T, Hkv, D).transpose(1, 2)
@@ -285,22 +309,10 @@ def test_rope_kv_append(ops):
     orig = qkv.clone()
     k_cache = torch.zeros((B, Hkv, Tmax, D), device="cuda", dtype=bf16)
     v_cache = torch.zeros_like(k_cache)
-    inv_freq = 1.0 / (theta ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))
+    inv_freq = (1.0 / (theta ** (torch.arange(0, D, 2, dtype=torch.int64).float() / D))).cuda()
     starts = torch.tensor([0, 9], dtype=torch.int32, device="cuda")
-    ops.rope_kv_append(qkv, k_cache, v_cache, B=B, T=T, H=H, Hkv=Hkv, D=D, pos0=0, inv_freq=inv_freq.cuda(), kv_start=starts)
-    pos = (torch.arange(T, device="cuda")[None, :] - starts[:, None]).clamp(min=-1)
-    pos = torch.where(pos < 0, torch.ones_like(pos), pos).float()  # padded -> 1
-    freqs = pos[:, :, None] * inv_freq.cuda()[None, None, :]
-    emb = torch.cat([freqs, freqs], -1)
-    cos, sin = emb.cos().to(bf16), emb.sin().to(bf16)
-
-    def rot(x):  # x [B,T,h,D] bf16, reference op order with bf16 rounding at every op
-        x1, x2 = x[..., : D // 2], x[..., D // 2:]
-        rh = torch.cat([-x2, x1], -1)
-        return x * cos[:, :, None, :] + rh * sin[:, :, None, :]
-
-    o = orig.view(B, T, H + 2 * Hkv, D)
-    q_ref, k_ref, v_ref = rot(o[:, :, :H]), rot(o[:, :, H:H + Hkv]), o[:, :, H + Hkv:]
+    ops.rope_kv_append(qkv, k_cache, v_cache, B=B, T=T, H=H, Hkv=Hkv, D=D, pos0=0, inv_freq=inv_freq, kv_start=starts)
+    q_ref, k_ref, v_ref = rope_reference(orig, B, T, H, Hkv, D, 0, inv_freq, starts)
     got = qkv.view(B, T, H + 2 * Hkv, D)
     assert (got[:, :, :H].float() - q_ref.float()).abs().max().item() <= 2 ** -6 * q_ref.float().abs().max().item()
     frac_exact = (got[:, :, :H] == q_ref).float().mean().item()
@@ -310,18 +322,28 @@ def test_rope_kv_append(ops):
 
 
 @pytest.mark.parametrize(
-    "B,H,Hkv,Tmax,ctx,starts,splits",
+    "B,H,Hkv,Tmax,ctx,starts,splits,scores",
     [
-        (3, 28, 4, 1024, 777, [0, 100, 776], None),   # auto: one chunk per split
-        (3, 28, 4, 1024, 777, [0, 100, 776], 1),      # one CTA streams 7 chunks (ring wraps twice)
-        (3, 28, 4, 1024, 777, [0, 100, 776], 3),      # 3 / 3 / 1 chunks; row 2 has a single live key
-        (2, 16, 1, 2048, 1901, [5, 1300], 1),         # G = 16 (no padded heads), 15 chunks in one CTA
-        (2, 8, 4, 2048, 1537, [0, 640], 5),           # G = 2, uneven splits, last chunk holds one key
-        (40, 28, 4, 512, 300, None, None),            # B * Hkv > SM count -> nz = 1, more CTAs than SMs
-        (1, 28, 4, 128, 1, [0], None),                # a single key
+        (3, 28, 4, 1024, 777, [0, 100, 776], None, "random"),   # auto: one chunk per split
+        (3, 28, 4, 1024, 777, [0, 100, 776], 1, "random"),      # one CTA streams 7 chunks (ring wraps twice)
+        (3, 28, 4, 1024, 777, [0, 100, 776], 3, "random"),      # 3 / 3 / 1 chunks; row 2 has a single live key
+        (2, 16, 1, 2048, 1901, [5, 1300], 1, "random"),         # G = 16 (no padded heads), 15 chunks in one CTA
+        (2, 8, 4, 2048, 1537, [0, 640], 5, "random"),           # G = 2, uneven splits, last chunk holds one key
+        (40, 28, 4, 512, 300, None, None, "random"),            # B * Hkv > SM count -> nz = 1, more CTAs than SMs
+        (1, 28, 4, 128, 1, [0], None, "random"),                # a single key
+        (2, 4, 4, 1024, 700, [0, 300], None, "random"),         # G = 1: seven padded heads of NG = 8
+        (2, 4, 4, 1024, 700, [0, 300], 3, "random"),
+        (2, 32, 4, 1024, 700, [0, 300], None, "random"),        # G = 8: the widest NG = 8 group
+        (2, 32, 4, 1024, 700, [0, 300], 3, "random"),
+        (2, 36, 4, 1024, 700, [0, 300], None, "random"),        # G = 9: the narrowest NG = 16 group
+        (2, 36, 4, 1024, 700, [0, 300], 3, "random"),
+        (2, 28, 4, 2048, 1901, [0, 300], 1, "rising"),          # running max moves every chunk inside one CTA
+        (2, 28, 4, 2048, 1901, [0, 300], None, "rising"),       # ... and across the split partials (one chunk each)
+        (2, 28, 4, 2048, 1901, [0, 300], 3, "falling"),         # maximum in the first chunk
+        (2, 28, 4, 2048, 1901, [5, 1300], 4, "two_peaks"),      # equal peaks in the first and the last split
     ],
 )
-def test_decode_attention(ops, monkeypatch, B, H, Hkv, Tmax, ctx, starts, splits):
+def test_decode_attention(ops, monkeypatch, B, H, Hkv, Tmax, ctx, starts, splits, scores):
     D = 128
     if splits is None:
         monkeypatch.delenv("AF3_DECODE_SPLITS", raising=False)
@@ -330,6 +352,11 @@ def test_decode_attention(ops, monkeypatch, B, H, Hkv, Tmax, ctx, starts, splits
     qkv = _rand((B, (H + 2 * Hkv) * D), 1.0, 43)
     k_cache, v_cache = _rand((B, Hkv, Tmax, D), 1.0, 44), _rand((B, Hkv, Tmax, D), 1.0, 45)
     starts_t = torch.tensor(starts if starts is not None else [0] * B, dtype=torch.int32, device="cuda")
+    for b in range(B):
+        first = int(starts_t[b]) + (3 if scores == "two_peaks" else 0)
+        last = ctx - (4 if scores == "two_peaks" else 1)
+        _peak_scores(qkv[b, :H * D].view(H, D), k_cache[b], scores, D ** -0.5, first, last,
+                     torch.arange(Tmax, device="cuda", dtype=torch.float32)[None, :])
     ctx_len = torch.tensor([ctx], dtype=torch.int32, device="cuda")
     out = torch.zeros((B, H * D), device="cuda", dtype=bf16)
     scratch = ops.decode_attention_scratch(B, H, D, Tmax, "cuda")
@@ -384,14 +411,7 @@ def test_logmel_vs_fp64(ops):
     wave = (rs.randn(2, n) * 0.1).astype(np.float32)
     wave[1, 160000:] = 0.0  # zero-padded short clip
     got = ops.logmel(torch.from_numpy(wave).cuda(), tables).cpu().numpy()
-    # fp64 reference
-    win = torch.hann_window(400, dtype=torch.float64)
-    st = torch.stft(torch.from_numpy(wave).double(), 400, 160, window=win, return_complex=True)
-    mag = st[..., :-1].abs() ** 2
-    mel = torch.from_numpy(filt).double().T @ mag
-    ls = torch.clamp(mel, min=1e-10).log10()
-    mx = ls.amax(dim=(1, 2), keepdim=True)
-    ref = ((torch.maximum(ls, mx - 8.0) + 4.0) / 4.0).numpy()
+    ref = logmel_reference(wave, filt)
     err = np.abs(got - ref)
     assert got.shape == (2, 128, 3000)
     assert err.max() < 1e-4, err.max()
