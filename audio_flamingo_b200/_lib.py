@@ -44,6 +44,8 @@ SIGNATURES = {
     "af3_embed_scatter": (_i, [_p, _p, _i, _p, _i, _i64, _p, _i, _i, _p, _p, _p, _p]),
     "af3_argmax_scratch_bytes": (_sz, [_i]),
     "af3_argmax": (_i, [_p, _p, _i, _i, _p, _p]),
+    "af3_logits_process_scratch_bytes": (_sz, [_i, _i]),
+    "af3_logits_process_argmax": (_i, [_p, _p, _i, _i, _p, _p, _i, _p, _p, _p, _i, _p, _p, _p]),
     "af3_token_step": (_i, [_p, _p, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
     "af3_quant_fp8": (_i, [_p, _p, _i, _p, _p, _i, _i]),
     "af3_gemm_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _sz]),

@@ -30,6 +30,9 @@ int embed_scatter(cudaStream_t, const int64_t*, int, const bf16*, int, int64_t, 
                   int*, int*);
 int argmax(cudaStream_t, const float*, int, int, int64_t*, void*);
 size_t argmax_scratch_bytes(int B);
+size_t logits_process_scratch_bytes(int B, int cap);
+int logits_process_argmax(cudaStream_t, const float*, int, int, const int64_t*, const int64_t*, int, const int*, const int*, const float*, int,
+                          float*, int64_t*, void*);
 int attention(cudaStream_t stream, const bf16* q, int ldq, const bf16* k, const bf16* v, int ldk, int kv_layout,
               int Tk_pitch, bf16* out, int ldo, int B, int H, int Hkv, int D, int Tq, int Tk, float scale, int causal,
               const int* kv_len, const int* kv_start);
@@ -183,6 +186,13 @@ int af3_token_step(void* stream, const int64_t* raw_ids, int B, int* unfinished,
 size_t af3_argmax_scratch_bytes(int B) { return af3::argmax_scratch_bytes(B); }
 int af3_argmax(void* stream, const float* logits, int B, int V, int64_t* out_ids, void* scratch) {
     return af3::argmax(S(stream), logits, B, V, out_ids, scratch);
+}
+size_t af3_logits_process_scratch_bytes(int B, int cap) { return af3::logits_process_scratch_bytes(B, cap); }
+int af3_logits_process_argmax(void* stream, const float* logits, int B, int V, const int64_t* prompt_ids, const int64_t* generated_ids,
+                              int ld_ids, const int* gen_idx, const int* tables, const float* static_add, int cap, float* scores,
+                              int64_t* out_ids, void* scratch) {
+    return af3::logits_process_argmax(S(stream), logits, B, V, prompt_ids, generated_ids, ld_ids, gen_idx, tables, static_add, cap, scores,
+                                      out_ids, scratch);
 }
 
 }  // extern "C"

@@ -862,4 +862,249 @@ int token_step(cudaStream_t stream, const int64_t* raw_ids, int B, int* unfinish
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Greedy logits processors + selection (include/af3b200.h af3_logits_process_argmax), the device restatement of
+// [O] generation/logits_process.py SequenceBias, NoRepeatNGram, NoBadWords, MinLength, MinNewTokensLength, ForcedEOSToken,
+// SuppressTokens and SuppressTokensAtBegin in the order of [O] generation/utils.py _get_logits_processor.
+// Per row and step the processed value of token t is
+//   forced step  : 0 at the forced EOS ids (unless suppressed or begin-suppressed), -inf elsewhere
+//   otherwise    : -inf if any mask rule hits t, else x + bias_total(t)
+// Rules that depend on only the token (single-token bias, single-token bad words, suppress_tokens) sit in a dense fp32
+// vector static_add [V] (bias, or -inf); the rest depend on the history or the step and are found by logits_rules_kernel,
+// which writes a short per-row list of (token, kind, value).  logits_process_partial_kernel then reads each logit once,
+// adds static_add, overrides the listed tokens and reduces its slice to (max, first index) exactly like
+// argmax_partial_kernel; argmax_final_kernel merges the slices.  The list order is irrelevant to every output: mask bits are
+// OR-ed, a token has at most one ADD / SET entry, and (max, first index) merging is order-free.
+enum : int {
+    LP_S = 0, LP_NGRAM, LP_MINLEN, LP_MINNEW, LP_BEGIN, LP_FORCED, LP_STATIC,
+    LP_NEOS, LP_OEOS, LP_NBEGIN, LP_OBEGIN, LP_NFORCED, LP_OFORCED, LP_NBAD, LP_OBAD, LP_NGRP, LP_OGRP,
+    LP_HDR = 32
+};
+enum : int { LP_MASK = 0, LP_ADD = 1, LP_SET = 2 };
+constexpr int LP_MAXW = 1024;   // bitmap words per slice -> slices of up to 32768 tokens
+
+__device__ __forceinline__ int64_t lp_hist(const int64_t* __restrict__ prompt, const int64_t* __restrict__ gen, size_t off, int S,
+                                           int t) {
+    return t < S ? __ldg(prompt + off + t) : gen[off + (t - S)];
+}
+
+__device__ __forceinline__ void lp_emit(int2* __restrict__ list, int cap, int* cnt, int tok, int kind, float val) {
+    const int s = atomicAdd(cnt, 1);   // slot allocation only; see the order note above
+    if (s < cap) list[s] = make_int2(static_cast<int>(static_cast<unsigned>(tok) | (static_cast<unsigned>(kind) << 30)), __float_as_int(val));
+}
+
+// One CTA per row.  History = prompt[b][0, S) followed by generated[b][0, *gen_idx): the input_ids the reference's processors see.
+__global__ void __launch_bounds__(256)
+logits_rules_kernel(const int64_t* __restrict__ prompt, const int64_t* __restrict__ generated, int ld, int V, const int* __restrict__ gen_idx,
+                    const int* __restrict__ tab, int2* __restrict__ list, int2* __restrict__ row_info, int cap, unsigned long long* trace) {
+    if (threadIdx.x == 0) trace_mark(trace, 0);
+    pdl_launch_dependents();
+    pdl_wait();
+    if (threadIdx.x == 0) trace_mark(trace, 1);
+    __shared__ int h[LP_HDR];
+    __shared__ int cnt;
+    if (threadIdx.x < LP_HDR) h[threadIdx.x] = tab[threadIdx.x];
+    if (threadIdx.x == 0) cnt = 0;
+    __syncthreads();
+    const int b = blockIdx.x;
+    const int S = h[LP_S], gen = *gen_idx, cur = S + gen;
+    const size_t off = static_cast<size_t>(b) * ld;
+    int2* out = list + static_cast<size_t>(b) * cap;
+    const bool forced = h[LP_FORCED] >= 0 && cur == h[LP_FORCED];
+    const bool begin = cur == h[LP_BEGIN];
+    if (forced) {   // ForcedEOSToken assigns the row; only SuppressTokens / SuppressTokensAtBegin come after it
+        for (int r = threadIdx.x; r < h[LP_NFORCED]; r += blockDim.x) {
+            const int* f = tab + h[LP_OFORCED] + 2 * r;
+            const bool sup = (f[1] & 1) || ((f[1] & 2) && begin);
+            lp_emit(out, cap, &cnt, f[0], LP_SET, sup ? -INFINITY : 0.f);
+        }
+    } else {
+        // NoRepeatNGram: every earlier n-gram whose first n-1 tokens equal the last n-1 tokens bans its last token
+        const int n = h[LP_NGRAM];
+        if (n > 0 && cur + 1 >= n) {
+            const int p0 = cur - n + 1;
+            for (int j = threadIdx.x; j <= cur - n; j += blockDim.x) {
+                bool hit = true;
+                for (int k = 0; k < n - 1 && hit; ++k) hit = lp_hist(prompt, generated, off, S, j + k) == lp_hist(prompt, generated, off, S, p0 + k);
+                if (hit) {
+                    const int64_t t = lp_hist(prompt, generated, off, S, j + n - 1);
+                    if (t >= 0 && t < V) lp_emit(out, cap, &cnt, static_cast<int>(t), LP_MASK, -INFINITY);
+                }
+            }
+        }
+        // NoBadWords, sequences of 2+ tokens: the last token is banned when the history ends with the others
+        for (int r = threadIdx.x; r < h[LP_NBAD]; r += blockDim.x) {
+            const int* rec = tab + h[LP_OBAD] + 2 * r;
+            const int* seq = tab + rec[0];
+            const int L = rec[1];
+            if (L > cur) continue;
+            bool hit = true;
+            for (int k = 0; k < L - 1 && hit; ++k) hit = lp_hist(prompt, generated, off, S, cur - L + 1 + k) == seq[k];
+            if (hit) lp_emit(out, cap, &cnt, seq[L - 1], LP_MASK, -INFINITY);
+        }
+        // SequenceBias, sequences of 2+ tokens, grouped by last token: 0 + single-token bias + every matching sequence's bias
+        // in dict order, one fp32 add each (the reference's bias tensor accumulation)
+        for (int r = threadIdx.x; r < h[LP_NGRP]; r += blockDim.x) {
+            const int* g = tab + h[LP_OGRP] + 4 * r;
+            float total = 0.f + __int_as_float(g[1]);
+            bool any = false;
+            for (int m = 0; m < g[3]; ++m) {
+                const int* mem = tab + g[2] + 3 * m;
+                const int* seq = tab + mem[0];
+                const int L = mem[1];
+                if (L > cur) continue;
+                bool hit = true;
+                for (int k = 0; k < L - 1 && hit; ++k) hit = lp_hist(prompt, generated, off, S, cur - L + 1 + k) == seq[k];
+                if (hit) {
+                    total += __int_as_float(mem[2]);
+                    any = true;
+                }
+            }
+            if (any) lp_emit(out, cap, &cnt, g[0], LP_ADD, total);
+        }
+        // MinLength (counts the prompt) and MinNewTokensLength (counts generated tokens) mask the EOS ids
+        if (cur < h[LP_MINLEN] || gen < h[LP_MINNEW])
+            for (int r = threadIdx.x; r < h[LP_NEOS]; r += blockDim.x) lp_emit(out, cap, &cnt, tab[h[LP_OEOS] + r], LP_MASK, -INFINITY);
+        if (begin)
+            for (int r = threadIdx.x; r < h[LP_NBEGIN]; r += blockDim.x) lp_emit(out, cap, &cnt, tab[h[LP_OBEGIN] + r], LP_MASK, -INFINITY);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        row_info[b] = make_int2(min(cnt, cap), forced ? 1 : 0);
+        trace_mark(trace, 3);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+logits_process_partial_kernel(const float* __restrict__ logits, int V, const float* __restrict__ static_add, const int* __restrict__ tab,
+                              const int2* __restrict__ list, const int2* __restrict__ row_info, int cap, float* __restrict__ scores,
+                              float* __restrict__ pmax, int* __restrict__ pidx, unsigned long long* trace) {
+    if (threadIdx.x == 0) trace_mark(trace, 0);
+    pdl_launch_dependents();
+    __shared__ unsigned ovr[LP_MAXW];   // token of the slice has a list entry
+    __shared__ unsigned msk[LP_MAXW];   // ... and one of them is a mask
+    const int row = blockIdx.x, sp = blockIdx.y;
+    const int per = ((V + AM_SPLIT - 1) / AM_SPLIT + 3) & ~3;
+    const int beg = sp * per, end = min(V, beg + per);
+    const int nw = (per + 31) >> 5;
+    for (int w = threadIdx.x; w < nw; w += blockDim.x) ovr[w] = msk[w] = 0u;
+    pdl_wait();
+    if (threadIdx.x == 0) trace_mark(trace, 1);
+    const bool has_static = tab[LP_STATIC] != 0;
+    const int2 info = row_info[row];
+    const int n = info.x;
+    const bool forced = info.y != 0;
+    const int2* ent = list + static_cast<size_t>(row) * cap;
+    __syncthreads();
+    for (int e = threadIdx.x; e < n; e += blockDim.x) {
+        const int2 en = ent[e];
+        const int t = en.x & 0x3fffffff;
+        if (t < beg || t >= end) continue;
+        const unsigned bit = 1u << ((t - beg) & 31);
+        atomicOr(&ovr[(t - beg) >> 5], bit);
+        if ((static_cast<unsigned>(en.x) >> 30) == LP_MASK) atomicOr(&msk[(t - beg) >> 5], bit);
+    }
+    __syncthreads();
+    const float* p = logits + static_cast<size_t>(row) * V;
+    float* so = scores ? scores + static_cast<size_t>(row) * V : nullptr;
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    const bool vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(so) | reinterpret_cast<uintptr_t>(static_add)) & 15) == 0;
+    int tail = beg;
+    if (vec) {
+        const int n4 = max(end - beg, 0) / 4;
+        for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+            const int rel = 4 * i, base = beg + rel;
+            const unsigned skip = (ovr[rel >> 5] >> (rel & 31)) & 0xFu;
+            float4 v = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+            if (!forced) {
+                v = __ldg(reinterpret_cast<const float4*>(p + base));
+                if (has_static) {
+                    const float4 s = __ldg(reinterpret_cast<const float4*>(static_add + base));
+                    v = make_float4(v.x + s.x, v.y + s.y, v.z + s.z, v.w + s.w);
+                }
+            }
+            if (!(skip & 1u)) argmax_merge(best, bi, v.x, base);
+            if (!(skip & 2u)) argmax_merge(best, bi, v.y, base + 1);
+            if (!(skip & 4u)) argmax_merge(best, bi, v.z, base + 2);
+            if (!(skip & 8u)) argmax_merge(best, bi, v.w, base + 3);
+            if (so) {
+                if (!skip) {
+                    *reinterpret_cast<float4*>(so + base) = v;
+                } else {
+                    if (!(skip & 1u)) so[base] = v.x;
+                    if (!(skip & 2u)) so[base + 1] = v.y;
+                    if (!(skip & 4u)) so[base + 2] = v.z;
+                    if (!(skip & 8u)) so[base + 3] = v.w;
+                }
+            }
+        }
+        tail = beg + n4 * 4;
+    }
+    for (int t = tail + threadIdx.x; t < end; t += blockDim.x) {
+        if ((ovr[(t - beg) >> 5] >> ((t - beg) & 31)) & 1u) continue;
+        const float v = forced ? -INFINITY : (has_static ? p[t] + __ldg(static_add + t) : p[t]);
+        argmax_merge(best, bi, v, t);
+        if (so) so[t] = v;
+    }
+    // listed tokens: a token listed more than once resolves to the same value from every entry
+    for (int e = threadIdx.x; e < n; e += blockDim.x) {
+        const int2 en = ent[e];
+        const int t = en.x & 0x3fffffff;
+        if (t < beg || t >= end) continue;
+        const int kind = static_cast<int>(static_cast<unsigned>(en.x) >> 30);
+        float v;
+        if (kind == LP_SET) {
+            v = __int_as_float(en.y);
+        } else if (kind == LP_MASK || ((msk[(t - beg) >> 5] >> ((t - beg) & 31)) & 1u)) {
+            v = -INFINITY;
+        } else {   // LP_ADD: a token masked in static_add stays masked whatever its sequence bias
+            const float s = has_static ? __ldg(static_add + t) : 0.f;
+            v = (s == -INFINITY) ? -INFINITY : p[t] + __int_as_float(en.y);
+        }
+        argmax_merge(best, bi, v, t);
+        if (so) so[t] = v;
+    }
+    __shared__ float sb[8];
+    __shared__ int si[8];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) argmax_merge(best, bi, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bi, o));
+    if ((threadIdx.x & 31) == 0) {
+        sb[threadIdx.x >> 5] = best;
+        si[threadIdx.x >> 5] = bi;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < 8; ++w) argmax_merge(best, bi, sb[w], si[w]);
+        pmax[row * AM_SPLIT + sp] = best;
+        pidx[row * AM_SPLIT + sp] = bi;
+        trace_mark(trace, 3);
+    }
+}
+
+size_t logits_process_scratch_bytes(int B, int cap) {
+    return argmax_scratch_bytes(B) + static_cast<size_t>(B) * (static_cast<size_t>(cap) + 1) * sizeof(int2);
+}
+
+int logits_process_argmax(cudaStream_t stream, const float* logits, int B, int V, const int64_t* prompt, const int64_t* generated, int ld,
+                          const int* gen_idx, const int* tables, const float* static_add, int cap, float* scores, int64_t* out,
+                          void* scratch) {
+    if (B <= 0) return 0;
+    AF3_REQUIRE(logits && prompt && generated && gen_idx && tables && static_add && out && scratch, "logits_process_argmax: null argument");
+    AF3_REQUIRE(cap >= 1 && ld >= 1, "logits_process_argmax: cap and ld must be positive");
+    AF3_REQUIRE(V >= 1 && ((V + AM_SPLIT - 1) / AM_SPLIT + 3) / 4 * 4 <= LP_MAXW * 32, "logits_process_argmax: V too large");
+    float* pmax = static_cast<float*>(scratch);
+    int* pidx = reinterpret_cast<int*>(pmax + static_cast<size_t>(B) * AM_SPLIT);
+    int2* row_info = reinterpret_cast<int2*>(static_cast<char*>(scratch) + argmax_scratch_bytes(B));
+    int2* list = row_info + B;
+    AF3_CHECK_CUDA(launch_kernel(logits_rules_kernel, dim3(B), dim3(256), 0, stream, prompt, generated, ld, V, gen_idx, tables, list, row_info,
+                                 cap, trace_next_slot()));
+    AF3_CHECK_CUDA(launch_kernel(logits_process_partial_kernel, dim3(B, AM_SPLIT), dim3(256), 0, stream, logits, V, static_add, tables,
+                                 static_cast<const int2*>(list), static_cast<const int2*>(row_info), cap, scores, pmax, pidx,
+                                 trace_next_slot()));
+    AF3_CHECK_CUDA(launch_kernel(argmax_final_kernel, dim3(B), dim3(32), 0, stream, static_cast<const float*>(pmax),
+                                 static_cast<const int*>(pidx), out, trace_next_slot()));
+    return 0;
+}
+
 }  // namespace af3

@@ -25,7 +25,7 @@ from typing import Optional
 import torch
 from torch import nn
 
-from . import _lib, ops
+from . import _lib, logits_process, ops
 from ._lib import AF3Error
 
 bf16 = torch.bfloat16
@@ -43,6 +43,19 @@ except Exception:  # pragma: no cover - minimal stand-ins with the same field na
     class CausalLMOutputWithPast:  # type: ignore
         loss: Optional[torch.Tensor] = None
         logits: torch.Tensor = None
+        past_key_values: object = None
+
+try:
+    from transformers.generation.utils import GenerateDecoderOnlyOutput
+except Exception:  # pragma: no cover
+
+    @dataclass
+    class GenerateDecoderOnlyOutput:  # type: ignore
+        sequences: torch.Tensor = None
+        scores: Optional[tuple] = None
+        logits: Optional[tuple] = None
+        attentions: Optional[tuple] = None
+        hidden_states: Optional[tuple] = None
         past_key_values: object = None
 
 
@@ -824,11 +837,11 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
 
     # ---- greedy generation ([O] GEN:2131 generate -> GEN:2658 _sample with do_sample=False)
     _IGNORED_WHEN_GREEDY = ("temperature", "top_p", "top_k", "min_p", "typical_p")        # unused by the reference too when do_sample=False
-    _ACCEPTED_DEFAULTS = {"num_beams": 1, "num_return_sequences": 1, "repetition_penalty": 1.0, "no_repeat_ngram_size": 0,
-                          "length_penalty": 1.0, "use_cache": True, "return_dict_in_generate": False, "output_scores": False,
-                          "output_logits": False, "num_beam_groups": 1, "penalty_alpha": None, "min_new_tokens": None,
-                          "min_length": 0, "assistant_model": None, "streamer": None, "logits_processor": None,
-                          "stopping_criteria": None, "bad_words_ids": None, "suppress_tokens": None, "synced_gpus": None}
+    _ACCEPTED_DEFAULTS = {"num_beams": 1, "num_return_sequences": 1, "repetition_penalty": 1.0,
+                          "length_penalty": 1.0, "use_cache": True, "num_beam_groups": 1, "penalty_alpha": None,
+                          "assistant_model": None, "streamer": None, "logits_processor": None,
+                          "stopping_criteria": None, "synced_gpus": None}
+    _OUTPUT_OPTIONS = ("return_dict_in_generate", "output_scores", "output_logits")
 
     def _generation_default(self, name):
         gc = getattr(self, "generation_config", None)
@@ -842,7 +855,13 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
         """Greedy decoding with the reference's `generate` call surface (prompt included in the returned ids, AF3M:547-551).
         Defaults follow the reference: eos_token_id / pad_token_id / max_new_tokens / do_sample come from `generation_config`
         (argument, else `self.generation_config`) when not passed; finished rows are padded and the loop stops once every row
-        has produced EOS (GEN:2797-2805).  Options of the reference this path does not implement raise instead of being ignored."""
+        has produced EOS (GEN:2797-2805).  Options of the reference this path does not implement raise instead of being ignored.
+        Greedy logits processors (sequence_bias, no_repeat_ngram_size, bad_words_ids, min_length, min_new_tokens,
+        forced_eos_token_id, suppress_tokens, begin_suppress_tokens; argument, else `generation_config`) run on the device inside
+        the decode step (include/af3b200.h af3_logits_process_argmax) and apply to every selected token, the first one included.
+        return_dict_in_generate=True returns a GenerateDecoderOnlyOutput: `scores` (output_scores) holds the processed rows and
+        `logits` (output_logits) the raw ones, one [B, V] tensor per generated token; past_key_values is None (the decode cache is
+        kept internally, see release_decode_state)."""
         if generation_config is not None:
             saved, self.generation_config = getattr(self, "generation_config", None), generation_config
             try:
@@ -852,6 +871,8 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                                      use_cuda_graph=use_cuda_graph, return_logits=return_logits, prefill_chunk_size=prefill_chunk_size, **kwargs)
             finally:
                 self.generation_config = saved
+        proc_kw = {k: kwargs.pop(k) for k in list(kwargs) if k in logits_process.OPTIONS}
+        out_kw = {k: kwargs.pop(k) for k in list(kwargs) if k in self._OUTPUT_OPTIONS}
         for k, v in kwargs.items():
             if k in self._IGNORED_WHEN_GREEDY:
                 continue
@@ -882,6 +903,18 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             pad_token_id = self._generation_default("pad_token_id")
         if prefill_chunk_size is None:
             prefill_chunk_size = self._generation_default("prefill_chunk_size")
+        eos_list = None
+        if eos_token_id is not None:
+            eos_list = [int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id]
+            if pad_token_id is None:
+                pad_token_id = eos_list[0]                                                    # GEN: "Setting pad_token_id to eos_token_id"
+        outs = {k: bool(out_kw[k] if out_kw.get(k) is not None else self._generation_default(k)) for k in self._OUTPUT_OPTIONS}
+        want_scores = outs["return_dict_in_generate"] and outs["output_scores"]
+        want_logits = return_logits or (outs["return_dict_in_generate"] and outs["output_logits"])
+        Tmax = AF3KVCache.bucket(S + max_new_tokens)
+        # processor options are validated and compiled here, on the host, before anything is enqueued
+        procs = logits_process.compile_processors(logits_process.resolve_options(proc_kw, self._generation_default), eos_list, S,
+                                                  S + max_new_tokens, lm.vocab, Tmax)
         try:
             self._mark("start")
             x = self._prompt_embeds(input_ids, input_features, input_features_mask)
@@ -891,11 +924,14 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             # Cache capacity is rounded up to a multiple of 256 rows: the captured graph depends on the capacity (cache pitch in the
             # tensor maps, scratch sizes) but not on the prompt length, so prompts of different lengths that fall into the same
             # bucket reuse one cache + graph.  The kernels only ever touch the live rows, the extra capacity costs memory only.
-            Tmax = AF3KVCache.bucket(S + max_new_tokens)
             # the captured graph holds raw addresses: key it on the weight storages too, so a re-pack (load_reference_state_dict) or
-            # a move (.to()) can never leave a stale graph replaying against freed memory
+            # a move (.to()) can never leave a stale graph replaying against freed memory.  With processors on, the step launches
+            # the processor kernels instead of the plain argmax, on buffers whose sizes are bucketed capacities: those are keyed too
+            proc_spec = None
+            if procs is not None:
+                proc_spec = (logits_process.bucket(procs.cap), logits_process.bucket(procs.tables.size), want_scores)
             key = (B, Tmax, use_graph, os.environ.get("AF3_PDL", "1") != "0", str(dev), lm.lm_head.weight.data_ptr(),
-                   lm._packed[0][0].data_ptr(), lm._packed[-1][2].data_ptr())
+                   lm._packed[0][0].data_ptr(), lm._packed[-1][2].data_ptr(), proc_spec)
             st = self._decode_state
             if st is not None and st["key"] == key:
                 cache, step_fn = st["cache"], st["step"]       # same buffers -> the captured graph is valid as it stands
@@ -903,7 +939,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             else:
                 self._decode_state = st = None                 # free the previous shape's cache and graph first
                 cache = lm.new_cache(B, Tmax)
-                step_fn = self._decode_runner(B, cache, use_graph)
+                step_fn = self._decode_runner(B, cache, use_graph, proc_spec)
                 self._decode_state = {"key": key, "cache": cache, "step": step_fn}
             if prefill_chunk_size is not None and 0 < prefill_chunk_size < S:
                 # chunked prefill (GEN:3770-3806): the prompt embeddings (audio rows already scattered in) go through the decoder in
@@ -916,19 +952,27 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             else:
                 logits = lm.prefill(x, kv_start, cache, logits_to_keep=1).view(B, -1)           # GEN:3724 _prefill
             self._mark("prefill_done")
-            eos_list = None
-            if eos_token_id is not None:
-                eos_list = [int(eos_token_id)] if isinstance(eos_token_id, int) else [int(e) for e in eos_token_id]
-                if pad_token_id is None:
-                    pad_token_id = eos_list[0]                                                # GEN: "Setting pad_token_id to eos_token_id"
-            kept_logits = [logits.clone()] if return_logits else None
-            step_fn.begin(ops.argmax(logits), eos_list, pad_token_id)                         # GEN:2793
-            n_done = self._token_loop(step_fn, cache, kept_logits, eos_list is not None, max_new_tokens)
+            kept_logits = [logits.clone()] if want_logits else None
+            kept_scores = None
+            if procs is None:
+                first = ops.argmax(logits)                                                    # GEN:2793
+                if want_scores:
+                    kept_scores = [logits.clone()]                                            # no processor: scores are the logits
+            else:
+                step_fn.load_processors(input_ids, procs)
+                first = step_fn.process(logits)
+                if want_scores:
+                    kept_scores = [step_fn.scores.clone()]
+            step_fn.begin(first, eos_list, pad_token_id)
+            n_done = self._token_loop(step_fn, cache, kept_logits, eos_list is not None, max_new_tokens, kept_scores)
             out = torch.empty((B, S + n_done), device=dev, dtype=torch.int64)
             out[:, :S] = input_ids.to(dev)
             out[:, S:] = step_fn.tok_buf[:, :n_done]
             result = out
             self._mark("decode_done")
+            if outs["return_dict_in_generate"]:
+                return GenerateDecoderOnlyOutput(sequences=result, scores=tuple(kept_scores) if want_scores else None,
+                                                 logits=tuple(kept_logits) if outs["output_logits"] else None, past_key_values=None)
             if return_logits:
                 return result, torch.stack(kept_logits, 1)
             return result
@@ -942,7 +986,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
     MAX_EOS_IDS = 8      # size of the device-side EOS set (af3_token_step)
     EOS_CHECK_EVERY = 8  # tokens between host reads of the "every row finished" flag (the reference syncs every token)
 
-    def _token_loop(self, step_fn, cache, kept_logits, has_eos, max_new_tokens):
+    def _token_loop(self, step_fn, cache, kept_logits, has_eos, max_new_tokens, kept_scores=None):
         """Greedy loop ([O] GEN:2743-2809).  The per-token bookkeeping (pad finished rows, append, EOS mask, "all finished") runs on
         the device inside the decode step (af3_token_step), so one iteration is one graph replay and nothing else; the host reads the
         "all finished" flags every EOS_CHECK_EVERY tokens (the reference syncs every token).  Returns the number of tokens generated.
@@ -958,6 +1002,8 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                     self.stage_host_t.append(("tok", time.perf_counter()))
                 if kept_logits is not None:
                     kept_logits.append(logits.clone())
+                if kept_scores is not None:
+                    kept_scores.append(step_fn.scores.clone() if step_fn.scores is not None else logits.clone())
             if has_eos and ((i + 1) % self.EOS_CHECK_EVERY == 0 or i + 1 == max_new_tokens):
                 flags = step_fn.done_flags[: i + 1].cpu()                                   # GEN:2805, one sync per EOS_CHECK_EVERY tokens
                 if bool(flags.any()):
@@ -967,13 +1013,18 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                     break
         if kept_logits is not None:
             del kept_logits[n_done:]
+        if kept_scores is not None:
+            del kept_scores[n_done:]
         return n_done
 
-    def _decode_runner(self, B, cache, use_graph):
+    def _decode_runner(self, B, cache, use_graph, proc_spec=None):
         """Returns the step object of the greedy loop: begin(first_ids, eos_list, pad) arms the device-side state, step() enqueues one
         token (bookkeeping, embedding gather, 28 layers, head, argmax) and returns the fp32 logits [B, V] buffer of the next token,
         finish() enqueues the bookkeeping of the last token; tok_buf [B, cap] / done_flags [cap] receive the tokens and the "every
-        row finished" flags.  With use_graph the step is captured once in a CUDA graph and replayed; positions advance on the device."""
+        row finished" flags.  With use_graph the step is captured once in a CUDA graph and replayed; positions advance on the device.
+        proc_spec = (rule-list entries per row, table capacity, scores wanted) switches the argmax to the logits processors:
+        load_processors(input_ids, compiled) fills their device tables for one call, process(logits) selects the first token,
+        and `scores` [B, V] receives each step's processed row when scores are wanted."""
         lm = self.language_model
         dev = lm.lm_head.weight.device
         table = lm.model.embed_tokens.weight
@@ -989,6 +1040,17 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
         gen_idx = torch.zeros((1,), device=dev, dtype=torch.int32)
         done_flags = torch.zeros((cap,), device=dev, dtype=torch.int32)
         am_out = raw_ids
+        if proc_spec is not None:
+            list_cap, tab_cap, want_scores = proc_spec
+            hist = torch.zeros((B, cap), device=dev, dtype=torch.int64)           # prompt ids; generated ids are read from tok_buf
+            tables = torch.zeros((tab_cap,), device=dev, dtype=torch.int32)
+            static_add = torch.zeros((lm.vocab,), device=dev, dtype=torch.float32)
+            scores = torch.empty((B, lm.vocab), device=dev, dtype=torch.float32) if want_scores else None
+
+        def select(logits, out):
+            if proc_spec is None:
+                return ops.argmax(logits, out=out)
+            return ops.logits_process_argmax(logits, hist, tok_buf, gen_idx, tables, static_add, list_cap, out=out, scores=scores)
 
         use_pdl = os.environ.get("AF3_PDL", "1") != "0"
 
@@ -1004,7 +1066,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                 bookkeeping()
                 x, _ = ops.embed_scatter(ids_buf, table, -1, None, 0, 1, None)
                 logits = lm.decode_step(x, cache, scratch)
-                ops.argmax(logits, out=am_out)
+                select(logits, am_out)
                 return logits
             finally:
                 ops.PHASE = phase
@@ -1030,6 +1092,19 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                 ctl[1:2].fill_(int(pad_token_id) if pad_token_id is not None else 0)
                 for j in range(n_eos):
                     eos_dev[j:j + 1].fill_(int(eos_list[j]))
+
+            def load_processors(self_, input_ids, compiled):
+                # staged through pinned memory: a pageable copy would block the host until the queued work drains (see begin)
+                S = input_ids.shape[1]
+                src = input_ids if input_ids.is_cuda else input_ids.pin_memory()
+                hist[:, :S].copy_(src, non_blocking=True)
+                tables[: compiled.tables.size].copy_(torch.from_numpy(compiled.tables).pin_memory(), non_blocking=True)
+                static_add.copy_(torch.from_numpy(compiled.static_add).pin_memory(), non_blocking=True)
+
+            def process(self_, logits):
+                """Processed greedy selection of the first token (history = the prompt alone)."""
+                gen_idx.zero_()
+                return select(logits, None)
 
             def finish(self_):
                 phase, ops.PHASE = ops.PHASE, "decode"
@@ -1064,6 +1139,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
 
         st = Step()
         st.tok_buf, st.done_flags = tok_buf, done_flags
+        st.scores = scores if proc_spec is not None else None
         return st
 
 

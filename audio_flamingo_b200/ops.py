@@ -493,3 +493,29 @@ def argmax(logits, out=None):
         check(lib.af3_argmax(stream_ptr(), ptr(logits), B, V, ptr(out), ptr(scratch)), "af3_argmax")
     _count(2)
     return out
+
+
+def logits_process_argmax(logits, prompt_ids, generated_ids, gen_idx, tables, static_add, cap, out=None, scores=None):
+    """Greedy logits processors + argmax in one pass over the logits (include/af3b200.h af3_logits_process_argmax).
+    logits fp32 [B, V]; prompt_ids / generated_ids int64 [B, ld] (history = prompt_ids[:, :S] + generated_ids[:, :gen_idx]);
+    gen_idx int32 [1]; tables int32 and static_add fp32 [V] from logits_process.compile_processors; scores: optional fp32
+    [B, V] that receives the processed rows."""
+    lib = _lib.load()
+    _req(logits, torch.float32, "logits"), _req(prompt_ids, torch.int64, "prompt_ids"), _req(generated_ids, torch.int64, "generated_ids")
+    _req(gen_idx, torch.int32, "gen_idx"), _req(tables, torch.int32, "tables"), _req(static_add, torch.float32, "static_add")
+    B, V = logits.shape
+    ld = prompt_ids.shape[1]
+    if generated_ids.shape != prompt_ids.shape or prompt_ids.shape[0] != B or static_add.numel() != V:
+        raise _lib.AF3Error("logits_process_argmax: prompt_ids / generated_ids must be [B, ld] and static_add [V]")
+    if scores is not None:
+        _req(scores, torch.float32, "scores")
+        if tuple(scores.shape) != (B, V):
+            raise _lib.AF3Error("logits_process_argmax: scores must be [B, V]")
+    if out is None:
+        out = torch.empty((B,), device=logits.device, dtype=torch.int64)
+    scratch = torch.empty((lib.af3_logits_process_scratch_bytes(B, cap),), device=logits.device, dtype=torch.uint8)
+    with _Timed(("logits_process", B, V, cap, int(scores is not None))):
+        check(lib.af3_logits_process_argmax(stream_ptr(), ptr(logits), B, V, ptr(prompt_ids), ptr(generated_ids), ld, ptr(gen_idx), ptr(tables),
+                                            ptr(static_add), cap, ptr(scores), ptr(out), ptr(scratch)), "af3_logits_process_argmax")
+    _count(3)
+    return out

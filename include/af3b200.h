@@ -196,6 +196,24 @@ int af3_embed_scatter(void* stream, const int64_t* ids, int n_tok, const void* e
 size_t af3_argmax_scratch_bytes(int B);
 int af3_argmax(void* stream, const float* logits, int B, int V, int64_t* out_ids, void* scratch);
 
+/* Greedy logits processors + selection in one pass over the logits: the chain [O] generation/utils.py:1037-1192
+ * _get_logits_processor builds for greedy decoding, restated from [O] generation/logits_process.py -- SequenceBiasLogitsProcessor,
+ * NoRepeatNGramLogitsProcessor, NoBadWordsLogitsProcessor, MinLengthLogitsProcessor, MinNewTokensLengthLogitsProcessor,
+ * ForcedEOSTokenLogitsProcessor, SuppressTokensLogitsProcessor, SuppressTokensAtBeginLogitsProcessor, in that order -- followed
+ * by the selection of af3_argmax (first index of the processed row's maximum, NaNs skipped, an all -inf row yields 0).
+ * The history the rules see is prompt_ids[b][0, S) followed by generated_ids[b][0, *gen_idx) (row pitch ld_ids for both), S
+ * taken from the tables; every per-call quantity lives in device memory, so the call can be captured in a CUDA graph.
+ * tables: int32 option tables written by audio_flamingo_b200.logits_process.compile_processors (header of 32 ints: S, n-gram
+ * size, min_length, min_new_tokens, begin index, forced-EOS length, static flag, then counts and offsets of the EOS, begin-suppress,
+ * forced-EOS, bad-word and sequence-bias records).  static_add fp32 [V]: every rule that depends on the token alone
+ * (single-token bias, or -inf for single-token bad words and suppress_tokens); read only when the static flag is set.
+ * cap: entries per row of the rule list (bounds the history-dependent hits).  scores (optional) fp32 [B, V] receives the
+ * processed rows.  scratch: af3_logits_process_scratch_bytes(B, cap) bytes. */
+size_t af3_logits_process_scratch_bytes(int B, int cap);
+int af3_logits_process_argmax(void* stream, const float* logits, int B, int V, const int64_t* prompt_ids, const int64_t* generated_ids,
+                              int ld_ids, const int* gen_idx, const int* tables, const float* static_add, int cap, float* scores,
+                              int64_t* out_ids, void* scratch);
+
 /* [O] generation/utils.py:2797-2805 (_sample, greedy): per generated token -- rows that have finished emit pad_token_id, the
  * token is appended, the unfinished mask is updated with the EOS set (EosTokenCriteria) and "every row finished" is published.
  * Device-side, so the whole token fits in the captured decode step.  raw_ids [B] (the argmax of the previous logits),
