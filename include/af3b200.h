@@ -136,7 +136,10 @@ int af3_rmsnorm(void* stream, const void* x, void* y, const void* weight, int ro
  * (b, t, hk*D + d) at k + (b*Tk + t)*ldk when kv_layout = 0 (packed projection buffer).
  * kv_len[b] (may be NULL = Tk): keys >= kv_len[b] are masked (AF3M:337-351 key padding).
  * kv_start[b] (may be NULL = 0): keys < kv_start[b] are masked (left padding, MASK:882).
- * causal: key j visible to query i iff j <= i + (Tk - Tq).   out[b, t, h*D + d] at out + (b*Tq + t)*ldo. */
+ * causal: key j visible to query i iff j <= i + (Tk - Tq).   out[b, t, h*D + d] at out + (b*Tq + t)*ldo.
+ * A query row with no visible key gets 0.  Rows at or past Tk are never read.  Masked keys inside a loaded 128-key tile
+ * (before kv_start[b], at or past kv_len[b]) are read: K may hold anything there, but V must be finite, because the
+ * tensor core multiplies it by P = 0 and 0 * NaN = NaN. */
 int af3_attention(void* stream, const void* q, int ldq, const void* k, const void* v, int ldk, int kv_layout,
                   int Tk_pitch, void* out, int ldo, int B, int H, int Hkv, int D, int Tq, int Tk, float scale,
                   int causal, const int* kv_len, const int* kv_start);

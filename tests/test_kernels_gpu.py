@@ -1,11 +1,12 @@
 """Per-kernel parity on the GPU: each C-ABI kernel against a plain torch fp32 restatement of the same op with the
 reference's bf16 rounding points (tolerances stated per test)."""
-import math
 
 import numpy as np
 import pytest
 import torch
 from test_cuda_core_kernels_gpu import logmel_reference, rope_reference
+from test_attention_kernels_gpu import (BIDIRECTIONAL, CAUSAL, CONTINUATION, DECODE_PORTED, bidirectional_case, causal_case,
+                                        check_decode, check_prefill, ported_decode_case)
 
 pytestmark = pytest.mark.gpu
 bf16 = torch.bfloat16
@@ -210,96 +211,26 @@ def test_conv_stem_as_gemm(ops):
     _close(h2.view(n_win, T // 2, Dm).permute(0, 2, 1), ref2, BF16_RTOL, 2e-3, "conv2")
 
 
-def _sdpa_ref(q, k, v, scale, mask):
-    # q [B,H,Tq,D], k/v [B,H,Tk,D] fp32; mask bool [B,1,Tq,Tk] True = visible
-    s = (q @ k.transpose(-1, -2)) * scale
-    s = s.masked_fill(~mask, float("-inf"))
-    p = torch.softmax(s, dim=-1)
-    p = torch.nan_to_num(p, nan=0.0)
-    return p @ v
-
-
-def _peak_scores(q, k, kind, scale, first, last, j):
-    """Overwrite q (every head = e_0) and k[..., 0] so that the attention score of the key at position j is a chosen profile
-    (natural-log units): 'rising' climbs by 20 per 128 keys up to the key at `last` (the running maximum moves every chunk and
-    the online-softmax rescale is << 1), 'falling' is its mirror (maximum at `first`), 'two_peaks' has equal peaks at `first` and
-    `last` and falls by 0.3 per key between them (partials whose maxima differ by hundreds).  'random' leaves both alone."""
-    if kind == "random":
-        return
-    if kind == "rising":
-        f = 20 / 128 * (j - last)
-    elif kind == "falling":
-        f = -20 / 128 * (j - first)
-    else:
-        f = -0.3 * torch.minimum((j - first).abs(), (j - last).abs())
-    q.zero_()
-    q[..., 0] = 1.0
-    k[..., 0] = (f / scale).to(k.dtype)
-
-
 @pytest.fixture(params=["v2", "v1"])
 def attn_impl(request, monkeypatch):
     """Both row tilings of the prefill / encoder attention kernel go through the same parity cases: v2 (two consumer warpgroups,
-    128 query rows per CTA = the default) and v1 (one warpgroup, 64 rows per CTA: AF3_ATTN_V1=1, kept as cross-check)."""
+    128 query rows per CTA = the default) and v1 (one warpgroup, 64 rows per CTA: AF3_ATTN_V1=1, kept as cross-check).
+    check_prefill runs both and requires identical bits; the parameter keeps the two halves of the case list apart."""
     monkeypatch.setenv("AF3_ATTN_V1", "1" if request.param == "v1" else "0")
     return request.param
 
 
-@pytest.mark.parametrize("D,H,T,lens", [(64, 4, 200, None), (64, 20, 1500, None), (64, 3, 333, [333, 100, 7]), (128, 2, 256, None),
-                                        (64, 2, 1500, [1500, 385, 12]), (128, 3, 700, [700, 129, 256]), (64, 2, 65, None),
-                                        (128, 2, 300, [300, 1, 190]), (64, 5, 2000, [2000, 1999, 640])])
-def test_attention_bidirectional(ops, attn_impl, D, H, T, lens):
-    B = 3 if lens else 2
-    qkv = _rand((B * T, 3 * H * D), 1.0, 40)
-    out = torch.zeros((B * T, H * D), device="cuda", dtype=bf16)
-    kv_len = torch.tensor(lens, dtype=torch.int32, device="cuda") if lens else None
-    ops.attention(qkv, qkv[:, H * D:], qkv[:, 2 * H * D:], out.view(B, T, H * D), B=B, H=H, Hkv=H, D=D, Tq=T, Tk=T,
-                  scale=0.125 if D == 64 else 128 ** -0.5, causal=False, kv_layout=0, ldq=3 * H * D, ldk=3 * H * D, kv_len=kv_len)
-    q, k, v = [t.float().view(B, T, H, D).transpose(1, 2) for t in qkv.split(H * D, dim=1)]
-    mask = torch.ones((B, 1, T, T), dtype=torch.bool, device="cuda")
-    if lens:
-        for b, L in enumerate(lens):
-            mask[b, :, :, L:] = False
-    ref = _sdpa_ref(q, k, v, 0.125 if D == 64 else 128 ** -0.5, mask).transpose(1, 2).reshape(B * T, H * D)
-    # P is rounded to bf16 before P.V (as in flash-style kernels) and O to bf16: ~2^-8 relative on O(1) values
-    _close(out, ref, 2e-2, 2e-2, f"attention D={D} T={T}")
+# The attention tests below run their cases through the checks of test_attention_kernels_gpu.py: the fp64 softmax bound, one
+# bf16 ulp from the tile / split restatement, a bit-identical floor, identical bits for both row tilings, poisoned memory the
+# kernel must mask, and output margins.
+@pytest.mark.parametrize("D,H,T,lens", BIDIRECTIONAL)
+def test_attention_bidirectional(ops, attn_impl, monkeypatch, D, H, T, lens):
+    check_prefill(ops, monkeypatch, bidirectional_case(D, H, T, lens))
 
 
-@pytest.mark.parametrize("T,starts,scores", [(256, None, "random"), (300, [0, 37, 250], "random"), (130, [5, 129], "random"),
-                                             (780, [0, 3, 530], "random"), (1000, None, "random"), (64, None, "random"),
-                                             (129, [0, 128], "random"), (513, [0, 400, 512], "random"),
-                                             (1000, [0, 3, 530], "rising"), (1000, [0, 3, 530], "falling"), (780, None, "two_peaks")])
-def test_attention_causal_gqa_cache(ops, attn_impl, T, starts, scores):
-    H, Hkv, D, Tmax = 8, 2, 128, 1024
-    B = len(starts) if starts else 2
-    qkv = _rand((B * T, (H + 2 * Hkv) * D), 1.0, 41)
-    tok = torch.arange(T, device="cuda", dtype=torch.float32).repeat(B)[:, None]
-    _peak_scores(qkv[:, :H * D].view(B * T, H, D), qkv[:, H * D:(H + Hkv) * D].view(B * T, Hkv, D), scores, D ** -0.5,
-                 T // 4, T - 1 if scores == "rising" else 3 * T // 4, tok)
-    k_cache = torch.zeros((B, Hkv, Tmax, D), device="cuda", dtype=bf16)
-    v_cache = torch.zeros_like(k_cache)
-    kk = qkv[:, H * D:(H + Hkv) * D].view(B, T, Hkv, D).transpose(1, 2)
-    vv = qkv[:, (H + Hkv) * D:].view(B, T, Hkv, D).transpose(1, 2)
-    k_cache[:, :, :T] = kk
-    v_cache[:, :, :T] = vv
-    out = torch.zeros((B * T, H * D), device="cuda", dtype=bf16)
-    kv_start = torch.tensor(starts, dtype=torch.int32, device="cuda") if starts else None
-    ops.attention(qkv, k_cache, v_cache, out.view(B, T, H * D), B=B, H=H, Hkv=Hkv, D=D, Tq=T, Tk=T, scale=D ** -0.5, causal=True,
-                  kv_layout=1, Tk_pitch=Tmax, ldq=(H + 2 * Hkv) * D, ldk=D, kv_start=kv_start)
-    q = qkv[:, :H * D].float().view(B, T, H, D).transpose(1, 2)
-    k = kk.float().repeat_interleave(H // Hkv, dim=1)
-    v = vv.float().repeat_interleave(H // Hkv, dim=1)
-    mask = torch.tril(torch.ones((T, T), dtype=torch.bool, device="cuda"))[None, None].repeat(B, 1, 1, 1)
-    if starts:
-        for b, s0 in enumerate(starts):
-            mask[b, :, :, :s0] = False
-    ref = _sdpa_ref(q, k, v, D ** -0.5, mask).transpose(1, 2).reshape(B * T, H * D)
-    valid = torch.ones((B, T), dtype=torch.bool, device="cuda")
-    if starts:
-        for b, s0 in enumerate(starts):
-            valid[b, :s0] = False
-    sel = valid.reshape(-1)
-    _close(out[sel], ref[sel], 2e-2, 2e-2, f"causal attention T={T}")
+@pytest.mark.parametrize("T,starts,scores", CAUSAL)
+def test_attention_causal_gqa_cache(ops, attn_impl, monkeypatch, T, starts, scores):
+    check_prefill(ops, monkeypatch, causal_case(T, starts, scores))
 
 
 def test_rope_kv_append(ops):
@@ -321,57 +252,9 @@ def test_rope_kv_append(ops):
     assert torch.equal(v_cache[:, :, :T].transpose(1, 2), v_ref)
 
 
-@pytest.mark.parametrize(
-    "B,H,Hkv,Tmax,ctx,starts,splits,scores",
-    [
-        (3, 28, 4, 1024, 777, [0, 100, 776], None, "random"),   # auto: one chunk per split
-        (3, 28, 4, 1024, 777, [0, 100, 776], 1, "random"),      # one CTA streams 7 chunks (ring wraps twice)
-        (3, 28, 4, 1024, 777, [0, 100, 776], 3, "random"),      # 3 / 3 / 1 chunks; row 2 has a single live key
-        (2, 16, 1, 2048, 1901, [5, 1300], 1, "random"),         # G = 16 (no padded heads), 15 chunks in one CTA
-        (2, 8, 4, 2048, 1537, [0, 640], 5, "random"),           # G = 2, uneven splits, last chunk holds one key
-        (40, 28, 4, 512, 300, None, None, "random"),            # B * Hkv > SM count -> nz = 1, more CTAs than SMs
-        (1, 28, 4, 128, 1, [0], None, "random"),                # a single key
-        (2, 4, 4, 1024, 700, [0, 300], None, "random"),         # G = 1: seven padded heads of NG = 8
-        (2, 4, 4, 1024, 700, [0, 300], 3, "random"),
-        (2, 32, 4, 1024, 700, [0, 300], None, "random"),        # G = 8: the widest NG = 8 group
-        (2, 32, 4, 1024, 700, [0, 300], 3, "random"),
-        (2, 36, 4, 1024, 700, [0, 300], None, "random"),        # G = 9: the narrowest NG = 16 group
-        (2, 36, 4, 1024, 700, [0, 300], 3, "random"),
-        (2, 28, 4, 2048, 1901, [0, 300], 1, "rising"),          # running max moves every chunk inside one CTA
-        (2, 28, 4, 2048, 1901, [0, 300], None, "rising"),       # ... and across the split partials (one chunk each)
-        (2, 28, 4, 2048, 1901, [0, 300], 3, "falling"),         # maximum in the first chunk
-        (2, 28, 4, 2048, 1901, [5, 1300], 4, "two_peaks"),      # equal peaks in the first and the last split
-    ],
-)
+@pytest.mark.parametrize("B,H,Hkv,Tmax,ctx,starts,splits,scores", DECODE_PORTED)
 def test_decode_attention(ops, monkeypatch, B, H, Hkv, Tmax, ctx, starts, splits, scores):
-    D = 128
-    if splits is None:
-        monkeypatch.delenv("AF3_DECODE_SPLITS", raising=False)
-    else:
-        monkeypatch.setenv("AF3_DECODE_SPLITS", str(splits))
-    qkv = _rand((B, (H + 2 * Hkv) * D), 1.0, 43)
-    k_cache, v_cache = _rand((B, Hkv, Tmax, D), 1.0, 44), _rand((B, Hkv, Tmax, D), 1.0, 45)
-    starts_t = torch.tensor(starts if starts is not None else [0] * B, dtype=torch.int32, device="cuda")
-    for b in range(B):
-        first = int(starts_t[b]) + (3 if scores == "two_peaks" else 0)
-        last = ctx - (4 if scores == "two_peaks" else 1)
-        _peak_scores(qkv[b, :H * D].view(H, D), k_cache[b], scores, D ** -0.5, first, last,
-                     torch.arange(Tmax, device="cuda", dtype=torch.float32)[None, :])
-    ctx_len = torch.tensor([ctx], dtype=torch.int32, device="cuda")
-    out = torch.zeros((B, H * D), device="cuda", dtype=bf16)
-    scratch = ops.decode_attention_scratch(B, H, D, Tmax, "cuda")
-    for _ in range(2):  # second call: the arrival counters must have been left at zero
-        out.zero_()
-        ops.decode_attention(qkv, k_cache, v_cache, out, scratch, B=B, H=H, Hkv=Hkv, D=D, ctx_len=ctx_len,
-                             kv_start=starts_t if starts is not None else None, scale=D ** -0.5)
-    q = qkv[:, :H * D].float().view(B, H, 1, D)
-    k = k_cache[:, :, :ctx].float().repeat_interleave(H // Hkv, dim=1)
-    v = v_cache[:, :, :ctx].float().repeat_interleave(H // Hkv, dim=1)
-    mask = torch.ones((B, 1, 1, ctx), dtype=torch.bool, device="cuda")
-    for b in range(B):
-        mask[b, :, :, :starts_t[b]] = False
-    ref = _sdpa_ref(q, k, v, D ** -0.5, mask).reshape(B, H * D)
-    _close(out, ref, 2e-2, 1e-2, "decode attention")
+    check_decode(ops, monkeypatch, ported_decode_case(B, H, Hkv, Tmax, ctx, starts, splits, scores))
 
 
 def test_embed_scatter_and_argmax(ops):
@@ -463,31 +346,9 @@ def test_qkv_rope_fused_gemm_never_writes_past_the_cache(ops):
 
 def test_attention_v2_matches_v1_on_a_live_cache_offset(ops, monkeypatch):
     """Continuation chunk (chunked prefill / next chat turn): Tq = 200 new rows against Tk = 650 cached + new keys, causal with the
-    (Tk - Tq) offset, GQA 28:4, left padding on one row.  The two kernel generations must agree to within bf16 output rounding, and
-    both with the fp32 restatement."""
-    B, H, Hkv, D, Tq, Tk, Tmax = 2, 28, 4, 128, 200, 650, 768
-    q = _rand((B * Tq, (H + 2 * Hkv) * D), 1.0, 90)
-    k_cache, v_cache = _rand((B, Hkv, Tmax, D), 1.0, 91), _rand((B, Hkv, Tmax, D), 1.0, 92)
-    k_cache[:, :, Tk:] = 0
-    v_cache[:, :, Tk:] = 0
-    kv_start = torch.tensor([0, 77], dtype=torch.int32, device="cuda")
-    outs = {}
-    for impl in ("0", "1"):
-        monkeypatch.setenv("AF3_ATTN_V1", impl)
-        out = torch.zeros((B * Tq, H * D), device="cuda", dtype=bf16)
-        ops.attention(q, k_cache, v_cache, out.view(B, Tq, H * D), B=B, H=H, Hkv=Hkv, D=D, Tq=Tq, Tk=Tk, scale=D ** -0.5, causal=True,
-                      kv_layout=1, Tk_pitch=Tmax, ldq=(H + 2 * Hkv) * D, ldk=D, kv_start=kv_start)
-        outs[impl] = out
-    qq = q[:, :H * D].float().view(B, Tq, H, D).transpose(1, 2)
-    kk = k_cache[:, :, :Tk].float().repeat_interleave(H // Hkv, dim=1)
-    vv = v_cache[:, :, :Tk].float().repeat_interleave(H // Hkv, dim=1)
-    qi = torch.arange(Tq, device="cuda")[:, None] + (Tk - Tq)
-    mask = (torch.arange(Tk, device="cuda")[None, :] <= qi)[None, None].repeat(B, 1, 1, 1)
-    mask[1, :, :, :77] = False
-    ref = _sdpa_ref(qq, kk, vv, D ** -0.5, mask).transpose(1, 2).reshape(B * Tq, H * D)
-    _close(outs["0"], ref, 2e-2, 2e-2, "v2 vs fp32")
-    _close(outs["1"], ref, 2e-2, 2e-2, "v1 vs fp32")
-    _close(outs["0"], outs["1"], 2 ** -6, 2e-3, "v2 vs v1")
+    (Tk - Tq) offset, GQA 28:4, left padding on one row.  The two row tilings give identical bits, and both meet the checks of
+    check_prefill."""
+    check_prefill(ops, monkeypatch, CONTINUATION)
 
 
 def test_token_step_is_the_references_per_token_rule(ops):
