@@ -49,6 +49,8 @@ SIGNATURES = {
     "af3_token_step": (_i, [_p, _p, _i, _p, _p, _p, _p, _i, _p, _p, _p]),
     "af3_quant_fp8": (_i, [_p, _p, _i, _p, _p, _i, _i]),
     "af3_gemm_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _sz]),
+    "af3_lm_head_xent_scratch_bytes": (_sz, [_i, _i]),
+    "af3_lm_head_xent": (_i, [_p, _p, _i, _p, _i, _i, _i, _i, _p, _i64, _p, _i, _p, _p, _p]),
     "af3_gemm_qkv_rope_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz]),
 }
 

@@ -120,6 +120,13 @@ int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_s
                          0, workspace, workspace_bytes, &r);
 }
 
+size_t af3_lm_head_xent_scratch_bytes(int n_tok, int V) { return af3::lm_head_xent_scratch_bytes(n_tok, V); }
+int af3_lm_head_xent(void* stream, const void* x, int ldx, const void* w, int ldw, int n_tok, int V, int K, const int64_t* labels,
+                     int64_t ignore_index, float* logits_out, int ldo, float* token_nll, double* totals, void* scratch) {
+    return af3::lm_head_xent(S(stream), B16(x), ldx, B16(w), ldw, n_tok, V, K, labels, ignore_index, logits_out, ldo, token_nll, totals,
+                             scratch);
+}
+
 int af3_pack_gate_up(void* stream, const void* gate, const void* up, void* packed, int F, int K) {
     return af3::pack_gate_up(S(stream), B16(gate), B16(up), B16M(packed), F, K);
 }

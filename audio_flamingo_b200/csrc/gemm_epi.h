@@ -6,7 +6,8 @@
 namespace af3 {
 
 enum : int { EPI_BIAS = 1, EPI_GELU = 2, EPI_RESID = 4, EPI_SWIGLU = 8, EPI_F32OUT = 16, EPI_ROPE = 32,
-              EPI_SWIGLU_CONCAT = 64 /* host-side only: weight rows are [gate; up], not interleaved (stripped before dispatch) */ };
+              EPI_SWIGLU_CONCAT = 64 /* host-side only: weight rows are [gate; up], not interleaved (stripped before dispatch) */,
+              EPI_XENT = 128 /* lm_head_xent only: softmax partials per (token, column tile), no output unless out != nullptr */ };
 
 // rotary embedding + KV-cache append in the epilogue of the few-token fused q/k/v projection
 struct RopeEpilogue {
@@ -27,5 +28,9 @@ int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, co
              void* out, int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res,
              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope);
 int quant_fp8(cudaStream_t stream, const bf16* x, int ldx, uint8_t* q, float* scales, int rows, int K);
+// LM head with the cross-entropy statistics in its epilogue (include/af3b200.h af3_lm_head_xent)
+size_t lm_head_xent_scratch_bytes(int n_tok, int V);
+int lm_head_xent(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, int n_tok, int V, int K, const int64_t* labels,
+                 int64_t ignore_index, float* logits_out, int ldo, float* token_nll, double* totals, void* scratch);
 
 }  // namespace af3

@@ -84,6 +84,11 @@ struct GemmArgs {
     const float* sx;
     const float* sw;
     int ld_sw;
+    // EPI_XENT (lm_head_xent): labels [n_tok] (shifted), one (max, sum exp) partial per (token, column tile) at
+    // xent_part[tok * num_c_tiles + c], the label's bf16-rounded logit at xent_tgt[tok]
+    const int64_t* labels;
+    float2* xent_part;
+    float* xent_tgt;
 };
 
 constexpr int BK = 64;  // 64 bf16 = 128 B = one swizzle atom row
@@ -415,6 +420,60 @@ __device__ __forceinline__ void epi_fragment(const float (&acc)[N / 2], const Ou
     }
 }
 
+// Cross-entropy epilogue of the 128 x 128 ping-pong kernel (EPI_XENT): softmax partials of the tile's 128 token rows over its
+// 128 columns, straight from the accumulator fragments, after the logits (if any) have been stored.  The accumulators are
+// rounded to bf16 in place, as the stored logits are, and set to -inf at columns >= V (exp gives 0).  A row's 128 columns are spread over the 4 lanes of a quad (32 each): (max, sum
+// exp(v - max)) per lane, then across the quad; lane 0 of the quad writes the partial.  The lane holding column labels[tok]
+// writes that logit: exactly one tile and one lane own a label in [0, V), none owns anything else.  Rows past n_tok (zero
+// filled by the TMA load) are skipped.
+__device__ __forceinline__ void xent_partials(float (&acc)[2][64], int r, int c, const GemmArgs& a) {
+    const int tw = threadIdx.x & 127;
+    const int lane = tw & 31;
+    const int frow = (tw >> 5) * 16 + (lane >> 2);
+    const int fcol = 2 * (lane & 3);
+    const int col0 = c * 128;
+    const int n_valid = a.n_feat - col0 - fcol;  // columns 8 cg + e of this lane below V: 8 cg + e < n_valid
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+            const int tok = r * 128 + h * 64 + frow + 8 * p;
+            const bool live = tok < a.n_tok;
+            float m = -INFINITY;
+#pragma unroll
+            for (int cg = 0; cg < 16; ++cg) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float& v = acc[h][4 * cg + 2 * p + e];
+                    v = 8 * cg + e < n_valid ? bf16_round(v) : -INFINITY;
+                    m = fmaxf(m, v);
+                }
+            }
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            float s = 0.f;
+#pragma unroll
+            for (int cg = 0; cg < 16; ++cg) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) s += __expf(acc[h][4 * cg + 2 * p + e] - m);
+            }
+            // the label's column within the tile, -1 unless it lies in this tile and below V
+            const long long lab = live ? a.labels[tok] : -1;
+            const int own = (lab >= col0 && lab < col0 + 128 && lab < a.n_feat) ? static_cast<int>(lab - col0) : -1;
+            float tgt = 0.f;
+#pragma unroll
+            for (int cg = 0; cg < 16; ++cg) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) tgt = 8 * cg + fcol + e == own ? acc[h][4 * cg + 2 * p + e] : tgt;
+            }
+            s += __shfl_xor_sync(0xffffffffu, s, 1);
+            s += __shfl_xor_sync(0xffffffffu, s, 2);
+            if (live && (lane & 3) == 0) a.xent_part[static_cast<size_t>(tok) * a.num_c_tiles + c] = make_float2(m, s);
+            if (own >= 0 && (own & 7) >> 1 == (lane & 3)) a.xent_tgt[tok] = tgt;
+        }
+    }
+}
+
 // ============================================================================ normal mode, 128 x 128 ping-pong tiles
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches); EPI < 0: generic instantiation reading
 // a.flags at run time (odd layouts / unusual flag mixes).
@@ -438,6 +497,8 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
     const int flags = (EPI >= 0) ? EPI : a.flags;
     const bool swiglu = flags & EPI_SWIGLU;
     const bool tma_res = a.tma_epi && (flags & EPI_RESID) && a.res_period == 0;
+    constexpr bool xent = EPI >= 0 && (EPI & EPI_XENT);
+    static_assert(!xent || EPI == (EPI_XENT | EPI_F32OUT), "the cross-entropy epilogue stores plain fp32 logits");
 
     // `empty`: 4 arrivals, one per warp of the warpgroup that consumes the tile; `order` barriers for the ping-pong
     if (threadIdx.x == 0) tok_prologue(sm, 4, true, a, &map_x, &map_w, &map_out, &map_res, a.tma_epi, tma_res);
@@ -509,8 +570,9 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
 
             // ---- epilogue from the accumulator fragments
             // the compile-time epilogues are launched only with the TMA-store path (gemm_bf16); the direct-store fallback
-            // exists in the generic instantiation alone, which keeps the specialised kernels small
-            if (EPI >= 0 || a.tma_epi) {
+            // exists in the generic instantiation alone, which keeps the specialised kernels small.  The cross-entropy
+            // epilogue (lm_head_xent) stores the fp32 logits by direct stores when a.out is set, then writes its partials.
+            if (!xent && (EPI >= 0 || a.tma_epi)) {
                 slabs.acquire(leader, tma_res, 1 + cw, &sm.rbar[cw], rpar);
                 // one unrolled pass over the tile per residual source, so that each pass holds only its own operands
                 auto stage_tile = [&](auto res_src) {
@@ -525,7 +587,7 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                 else
                     stage_tile(IntC<0>{});
                 slabs.store(leader, 1 + cw, &map_out, swiglu ? 1 : 2, out_col0, r * 128, a.n_feat);
-            } else {
+            } else if (!xent || a.out) {
                 // direct stores (output rows not 16-byte aligned, fp32 output): element pairs straight from the fragments
                 const int warp = tw >> 5, lane = tw & 31;
                 const int frow = warp * 16 + (lane >> 2);
@@ -578,6 +640,7 @@ gemm_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant
                     }
                 }
             }
+            if constexpr (xent) xent_partials(acc, r, c, a);  // after the store: the store's temporaries are dead by then
         }
         if (leader) bulk_wait_read<0>();  // staged tiles must be read out before shared memory goes away
     }
@@ -1477,6 +1540,106 @@ int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, co
         default:
             return fail("gemm_fp8: unsupported epilogue");
     }
+}
+
+// ============================================================================ LM head + cross-entropy (lm_head_xent)
+// A label is counted when it lies in [0, V) and is not ignore_index; one outside [0, V) that is not ignore_index is invalid:
+// never used as an index, counted as ignored and reported in totals[2].
+__device__ __forceinline__ bool xent_counted(long long lab, int V, long long ignore_index) { return lab >= 0 && lab < V && lab != ignore_index; }
+
+// One warp per token: lse from the token's column-tile partials, merged in a fixed order (lane j takes tiles j, j + 32, ...
+// in order, then a butterfly across the warp), and nll = lse - logit[label], 0 for an uncounted position.
+__global__ void __launch_bounds__(256)
+xent_merge_kernel(const float2* __restrict__ part, const float* __restrict__ tgt, const int64_t* __restrict__ labels, int n_tok,
+                  int n_ct, int V, long long ignore_index, float* __restrict__ token_nll) {
+    const int tok = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (tok >= n_tok) return;
+    if (!xent_counted(labels[tok], V, ignore_index)) {
+        if (lane == 0) token_nll[tok] = 0.f;
+        return;
+    }
+    const float2* p = part + static_cast<size_t>(tok) * n_ct;
+    float m = -INFINITY;
+    for (int j = lane; j < n_ct; j += 32) m = fmaxf(m, p[j].x);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float s = 0.f;
+    for (int j = lane; j < n_ct; j += 32) {
+        const float2 q = p[j];
+        s += q.y * expf(q.x - m);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) token_nll[tok] = m + logf(s) - tgt[tok];
+}
+
+// One CTA: totals = {sum of nll, counted positions, invalid labels}, in fp64 and a fixed order (thread i sums tokens i,
+// i + 1024, ..., then a tree over the threads).
+__global__ void __launch_bounds__(1024)
+xent_totals_kernel(const float* __restrict__ token_nll, const int64_t* __restrict__ labels, int n_tok, int V, long long ignore_index,
+                   double* __restrict__ totals) {
+    __shared__ double sh[3][1024];
+    double sum = 0.0, n = 0.0, bad = 0.0;
+    for (int t = threadIdx.x; t < n_tok; t += 1024) {
+        const long long lab = labels[t];
+        sum += token_nll[t];
+        n += xent_counted(lab, V, ignore_index) ? 1.0 : 0.0;
+        bad += (lab != ignore_index && (lab < 0 || lab >= V)) ? 1.0 : 0.0;
+    }
+    sh[0][threadIdx.x] = sum;
+    sh[1][threadIdx.x] = n;
+    sh[2][threadIdx.x] = bad;
+    __syncthreads();
+    for (int w = 512; w > 0; w >>= 1) {
+        if (threadIdx.x < w)
+            for (int k = 0; k < 3; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x < 3) totals[threadIdx.x] = sh[threadIdx.x][0];
+}
+
+// scratch: the partials [n_tok][ceil(V / 128)] float2, then the label logits [n_tok] float
+size_t lm_head_xent_scratch_bytes(int n_tok, int V) {
+    return static_cast<size_t>(n_tok) * ceil_div(V, 128) * sizeof(float2) + static_cast<size_t>(n_tok) * sizeof(float);
+}
+
+// Always the 128 x 128 ping-pong kernel, whatever n_tok: its k order is that of gemm_bf16's token-major fp32-output launch,
+// so stored logits equal what af3_gemm_bf16 returns for n_tok > 64, and the statistics do not depend on whether they are stored.
+int lm_head_xent(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, int n_tok, int V, int K, const int64_t* labels,
+                 int64_t ignore_index, float* logits_out, int ldo, float* token_nll, double* totals, void* scratch) {
+    AF3_REQUIRE(n_tok > 0 && V > 0 && K > 0, "lm_head_xent: empty problem");
+    AF3_REQUIRE((K % 8) == 0 && (ldx % 8) == 0 && (ldw % 8) == 0, "lm_head_xent: K and pitches must be multiples of 8");
+    AF3_REQUIRE(labels && token_nll && totals && scratch, "lm_head_xent: labels, token_nll, totals and scratch are required");
+    AF3_REQUIRE(!logits_out || ldo >= V, "lm_head_xent: ldo must be at least V");
+    GemmArgs a{};
+    a.K = K;
+    a.n_tok = n_tok;
+    a.n_feat = V;
+    a.out = logits_out;
+    a.ldo = ldo;
+    a.flags = EPI_XENT | EPI_F32OUT;
+    a.k_splits = 1;
+    a.trace = trace_next_slot();
+    a.num_r_tiles = ceil_div(n_tok, 128);
+    a.num_c_tiles = ceil_div(V, 128);
+    {  // rasterisation as gemm_bf16
+        const long long g = (20ll << 20) / (128ll * K * 2);
+        a.group_r = static_cast<int>(g < 8 ? 8 : (g > 256 ? 256 : g));
+    }
+    a.labels = labels;
+    a.xent_part = reinterpret_cast<float2*>(scratch);
+    a.xent_tgt = reinterpret_cast<float*>(a.xent_part + static_cast<size_t>(n_tok) * a.num_c_tiles);
+    CUtensorMap mx, mw;
+    if (int e = make_tmap_2d(&mx, x, K, n_tok, ldx, BK, 128)) return e;
+    if (int e = make_tmap_2d(&mw, w, K, V, ldw, BK, 128)) return e;
+    if (int e = launch_gemm<gemm_tok_kernel<TOK_STAGES, EPI_XENT | EPI_F32OUT>, TokCfg<TOK_STAGES>::SMEM_BYTES, TOK_THREADS>(a, stream, mx, mw, mx, mx))
+        return e;
+    xent_merge_kernel<<<ceil_div(n_tok, 8), 256, 0, stream>>>(a.xent_part, a.xent_tgt, labels, n_tok, a.num_c_tiles, V, ignore_index, token_nll);
+    AF3_CHECK_LAUNCH();
+    xent_totals_kernel<<<1, 1024, 0, stream>>>(token_nll, labels, n_tok, V, ignore_index, totals);
+    AF3_CHECK_LAUNCH();
+    return 0;
 }
 
 }  // namespace af3

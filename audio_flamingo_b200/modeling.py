@@ -59,6 +59,38 @@ except Exception:  # pragma: no cover
         past_key_values: object = None
 
 
+@dataclass
+class CausalLMOutputWithTokenLosses(CausalLMOutputWithPast):
+    """CausalLMOutputWithPast plus `token_losses`, fp32 [B, S]: the per-position negative log-likelihood whose mean is `loss`
+    (0 at ignored positions), so that candidates scored in one batch can be ranked by their row sums.  It is the last field:
+    .loss / .logits / .past_key_values and the leading tuple entries are the reference's."""
+
+    token_losses: Optional[torch.Tensor] = None
+
+
+def prepare_loss_labels(labels, shift_labels, ignore_index, B, S, V):
+    """The labels ForCausalLMLoss ([O] loss/loss_utils.py) compares the logits with: `labels` [B, S] padded with ignore_index
+    on the right and shifted left by one, or the caller's `shift_labels` [B, S] as they are.  -> int64 [B * S] on the labels'
+    device.  Integer [B, S] tensors only; host labels outside [0, V) other than ignore_index raise ValueError here (device
+    labels are checked by the kernel, which ignores them, and reported at the end of the call)."""
+    src = shift_labels if shift_labels is not None else labels
+    name = "shift_labels" if shift_labels is not None else "labels"
+    if not torch.is_tensor(src) or src.dtype.is_floating_point or src.dtype.is_complex or src.dtype == torch.bool:
+        raise ValueError(f"{name} must be an integer tensor")
+    if tuple(src.shape) != (B, S):
+        raise ValueError(f"{name} must have shape {(B, S)}, got {tuple(src.shape)}")
+    if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+        raise ValueError(f"ignore_index must be an int, got {ignore_index!r}")
+    src = src.to(torch.int64)
+    if shift_labels is None:
+        src = torch.nn.functional.pad(src, (0, 1), value=ignore_index)[:, 1:]
+    if not src.is_cuda:
+        bad = (src != ignore_index) & ((src < 0) | (src >= V))
+        if bool(bad.any()):
+            raise ValueError(f"{name} must lie in [0, {V}) or equal ignore_index ({ignore_index}); got {src[bad][:4].tolist()}")
+    return src.reshape(-1).contiguous()
+
+
 def _on_model_device(fn):
     """Runs a public entry point with the model's GPU as the current CUDA device: the C ABI launches on the current device
     (include/af3b200.h), so a model living on cuda:1 must not launch on cuda:0 (ADVICE r01)."""
@@ -514,11 +546,24 @@ class Qwen2ForCausalLM(nn.Module):
         y = ops.rmsnorm(h, self.model.norm.weight, self.eps, row_idx=row_idx)
         return ops.linear(y, self.lm_head.weight, out_f32=True)
 
+    def loss_head(self, y, labels, ignore_index=-100, num_items_in_batch=None, store_logits=False):
+        """LM head + ForCausalLMLoss on the post-norm hidden states y [n_tok, hid], with labels int64 [n_tok] already shifted
+        (prepare_loss_labels), without materialising the logits unless store_logits.  -> (fp32 logits [n_tok, V] or None,
+        token_losses fp32 [n_tok], loss 0-dim fp32, invalid-label count 0-dim).  loss = sum / counted positions, or sum /
+        num_items_in_batch when given, as fixed_cross_entropy; NaN when nothing is counted."""
+        logits, nll, totals = ops.lm_head_xent(y, self.lm_head.weight, labels, ignore_index, store_logits=store_logits)
+        n = totals[1] if num_items_in_batch is None else torch.as_tensor(num_items_in_batch, device=y.device).to(torch.float64)
+        return logits, nll, (totals[0] / n).to(torch.float32), totals[2]
+
     @torch.no_grad()
-    def prefill(self, inputs_embeds, kv_start, cache: AF3KVCache, logits_to_keep=1):
+    def prefill(self, inputs_embeds, kv_start, cache: AF3KVCache, logits_to_keep=1, labels=None, ignore_index=-100,
+                num_items_in_batch=None):
         """inputs_embeds [B,S,hid] bf16 (consumed in place), kv_start int32 [B]. -> fp32 logits [B, keep|S, V].
         The chunk is appended at cache.length (0 for a fresh prompt; > 0 for the next slice of a chunked prefill or a later chat turn:
-        RoPE positions, the causal offset and the left padding of the first chunk carry over)."""
+        RoPE positions, the causal offset and the left padding of the first chunk carry over).
+        With labels (int64 [B * S] on the device, already shifted): -> (logits or None, token_losses [B, S], loss, invalid-label
+        count), the loss over every position of the chunk whatever logits_to_keep.  With logits_to_keep = 0 the same launch
+        stores the logits; otherwise no [B, S, V] buffer exists."""
         self._check_ready()
         B, S, _ = inputs_embeds.shape
         if B != cache.B:
@@ -534,6 +579,17 @@ class Qwen2ForCausalLM(nn.Module):
         cache.length += S
         cache.pos_dev.fill_(cache.length)
         cache.ctx_dev.fill_(cache.length + 1)
+        if labels is not None:
+            if logits_to_keep not in (0, 1):
+                raise AF3Error("logits_to_keep must be 0 (all positions) or 1 (last position)")
+            y = ops.rmsnorm(h, self.model.norm.weight, self.eps)
+            logits, nll, loss, invalid = self.loss_head(y, labels, ignore_index, num_items_in_batch, store_logits=logits_to_keep == 0)
+            if logits_to_keep == 0:
+                logits = logits.view(B, S, self.vocab)
+            else:
+                last = torch.arange(B, device=h.device, dtype=torch.int32) * S + (S - 1)
+                logits = self._head(h, last).view(B, 1, self.vocab)
+            return logits, nll.view(B, S), loss, invalid
         if logits_to_keep == -1:  # an inner slice of a chunked prefill: only the cache is wanted
             return None
         if logits_to_keep == 0:
@@ -771,9 +827,14 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
             the chunk is appended at the cache's current length.  Its attention_mask -- [B, chunk] or the reference's
             full-length [B, past + chunk] -- must be all ones over the chunk (the kernels keep one contiguous live range per row).
         With use_cache the returned AF3KVCache has room for `reserve_tokens` more slots (default: up to the next multiple of 256)
-        and grows on demand in later calls, like DynamicCache."""
-        if labels is not None:
-            raise AF3Error("training (labels) is out of scope of the inference hot path")
+        and grows on demand in later calls, like DynamicCache.
+
+        Teacher-forced loss (inference only, no backward): with `labels` [B, S] (or `shift_labels`, used as they are) the output
+        carries `loss` as ForCausalLMLoss computes it -- keywords ignore_index (default -100) and num_items_in_batch as in the
+        reference -- and `token_losses` fp32 [B, S].  Both the prompt prefill and a continuation chunk take labels (covering
+        the chunk); the one-token cached step does not.  The loss covers every position whatever `logits_to_keep`, and is
+        computed in the LM head's epilogue without the [B, S, V] logits: with logits_to_keep=1 they are never allocated (the
+        memory-lean way to score), with logits_to_keep=0 the same launch also stores them."""
         if position_ids is not None:
             raise AF3Error("explicit position_ids are not supported; they are derived from the left-padded attention_mask")
         if (input_ids is None) == (inputs_embeds is None):
@@ -782,6 +843,24 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
         lm = self.language_model
         dev = lm.lm_head.weight.device
         cache = past_key_values
+        shift_labels = kwargs.get("shift_labels")
+        loss_kw = None
+        if labels is not None or shift_labels is not None:
+            B, S = (input_ids if input_ids is not None else inputs_embeds).shape[:2]
+            ignore_index = kwargs.get("ignore_index", -100)
+            if cache is not None and cache.length > 0 and inputs_embeds is None and input_features is None and S == 1:
+                raise AF3Error("labels on the one-token cached decode step are not implemented; pass them with the prompt or a longer chunk")
+            loss_kw = dict(labels=prepare_loss_labels(labels, shift_labels, ignore_index, B, S, lm.vocab).to(dev),
+                           ignore_index=ignore_index, num_items_in_batch=kwargs.get("num_items_in_batch"))
+
+        def output(res, cache_out):
+            if loss_kw is None:
+                return CausalLMOutputWithPast(logits=res, past_key_values=cache_out)
+            logits, token_losses, loss, invalid = res
+            self._defer_check(invalid != 0, ValueError,
+                              f"labels must lie in [0, {lm.vocab}) or equal ignore_index ({loss_kw['ignore_index']}): the invalid ones were ignored")
+            return CausalLMOutputWithTokenLosses(loss=loss, logits=logits, past_key_values=cache_out, token_losses=token_losses)
+
         try:
             if cache is not None and cache.length > 0:
                 single = inputs_embeds is None and input_features is None and input_ids.shape[1] == 1
@@ -812,8 +891,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                     elif bool(bad):
                         raise AF3Error(msg)
                 cache.ensure_capacity(cache.length + S + (reserve_tokens or 0))
-                logits = lm.prefill(inputs_embeds, None, cache, logits_to_keep=logits_to_keep)
-                return CausalLMOutputWithPast(logits=logits, past_key_values=cache)
+                return output(lm.prefill(inputs_embeds, None, cache, logits_to_keep=logits_to_keep, **(loss_kw or {})), cache)
             if inputs_embeds is None:
                 inputs_embeds = self._prompt_embeds(input_ids, input_features, input_features_mask)
             else:
@@ -828,8 +906,8 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                 cache = lm.new_cache(B, AF3KVCache.bucket(rows) if keep else max(S, 1))
             else:
                 cache.ensure_capacity(S + (reserve_tokens or 0))
-            logits = lm.prefill(inputs_embeds, kv_start, cache, logits_to_keep=logits_to_keep)
-            return CausalLMOutputWithPast(logits=logits, past_key_values=cache if keep else None)
+            return output(lm.prefill(inputs_embeds, kv_start, cache, logits_to_keep=logits_to_keep, **(loss_kw or {})),
+                          cache if keep else None)
         finally:
             self._raise_deferred()
 

@@ -111,6 +111,28 @@ def linear(x, w, bias=None, *, gelu=False, resid=None, res_period=0, out=None, o
     return out
 
 
+def lm_head_xent(x, w, labels, ignore_index=-100, *, store_logits=False):
+    """LM head with ForCausalLMLoss's cross-entropy in its epilogue (include/af3b200.h af3_lm_head_xent).  x [n_tok, K] bf16,
+    w [V, K] bf16, labels int64 [n_tok] already shifted.  -> (fp32 logits [n_tok, V] when store_logits else None, token_nll
+    fp32 [n_tok] (0 where uncounted), totals fp64 [3] = {sum of nll, counted positions, invalid labels})."""
+    lib = _lib.load()
+    _req(x, bf16, "x"), _req(w, bf16, "w"), _req(labels, torch.int64, "labels")
+    n_tok, K = x.shape
+    V = w.shape[0]
+    if labels.numel() != n_tok:
+        raise _lib.AF3Error(f"lm_head_xent: labels must hold one label per token ({n_tok}), got {labels.numel()}")
+    logits = torch.empty((n_tok, V), device=x.device, dtype=torch.float32) if store_logits else None
+    token_nll = torch.empty((n_tok,), device=x.device, dtype=torch.float32)
+    totals = torch.empty((3,), device=x.device, dtype=torch.float64)
+    scratch = torch.empty((lib.af3_lm_head_xent_scratch_bytes(n_tok, V),), device=x.device, dtype=torch.uint8)
+    with _Timed(("lm_head_xent", n_tok, V, K, int(store_logits))):
+        check(lib.af3_lm_head_xent(stream_ptr(), ptr(x), x.stride(0), ptr(w), w.stride(0), n_tok, V, K, ptr(labels), int(ignore_index),
+                                   ptr(logits), logits.stride(0) if logits is not None else 0, ptr(token_nll), ptr(totals), ptr(scratch)),
+              "af3_lm_head_xent")
+    _count(3)
+    return logits, token_nll, totals
+
+
 def pack_gate_up(gate, up):
     lib = _lib.load()
     _req(gate, bf16, "gate"), _req(up, bf16, "up")

@@ -105,6 +105,29 @@ int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_s
                           const float* rope_cs, void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace,
                           size_t workspace_bytes);
 
+/* ---- Teacher-forced loss: the LM head with the cross-entropy of [O] loss/loss_utils.py ForCausalLMLoss ->
+ * fixed_cross_entropy fused into its epilogue, without materialising the [n_tok, V] logits.  Additive (ABI v4).
+ *
+ * logits[t, v] = fp32(bf16( x[t,:] . w[v,:] )), the values af3_gemm_bf16 with AF3_EPI_F32OUT returns for n_tok > 64 (one
+ * 128 x 128 token-major tile kernel whatever n_tok, so for n_tok <= 64 they may differ from the few-token kernel's by the
+ * rounding of a different k order).  x bf16 [n_tok, K] (pitch ldx), w = lm_head.weight bf16 [V, K] (pitch ldw).
+ * labels int64 [n_tok]: the label of every position, ALREADY SHIFTED as ForCausalLMLoss shifts them (labels padded with
+ * ignore_index on the right and shifted left by one, or the caller's shift_labels).  A label is counted when it lies in
+ * [0, V) and differs from ignore_index; a label outside [0, V) that is not ignore_index is never used as an index: it is
+ * counted as ignored and reported (where the reference trips a device-side assert).
+ * Outputs: token_nll fp32 [n_tok] = logsumexp(logits[t]) - logits[t, labels[t]] at counted positions, 0 elsewhere;
+ * totals fp64 [3] = {sum of token_nll, counted positions, invalid labels}.  fixed_cross_entropy's loss is
+ * totals[0] / totals[1] (reduction "mean"; NaN with no counted position) or totals[0] / num_items_in_batch ("sum").
+ * logits_out (optional, fp32 [n_tok, V], pitch ldo >= V): the logits, stored by the same launch.
+ * Run to run bit-identical, and independent of whether logits_out is given.  Three launches: the GEMM (per token and 128-column
+ * tile: bf16-rounded values -> (max, sum exp(v - max)) in fp32; the tile holding the label column writes its logit), one warp
+ * per token merging its partials in column-tile order (fp32 lse), and a one-CTA fixed-order fp64 reduction into totals.
+ * scratch: af3_lm_head_xent_scratch_bytes(n_tok, V) = n_tok * (8 ceil(V / 128) + 4) bytes -- 237 MB at 24 960 tokens and
+ * V = 152 064, against 15.2 GB of fp32 logits. */
+size_t af3_lm_head_xent_scratch_bytes(int n_tok, int V);
+int af3_lm_head_xent(void* stream, const void* x, int ldx, const void* w, int ldw, int n_tok, int V, int K, const int64_t* labels,
+                     int64_t ignore_index, float* logits_out, int ldo, float* token_nll, double* totals, void* scratch);
+
 /* Log-mel front end; replaces WhisperFeatureExtractor._torch_extract_fbank_features ([O] WFE:135-164).
  * wave fp32 [n_win, n_samples] (zero padded to 30 s by the caller as WFE:296 does), mel_filters fp32 [201,128]
  * (from audio_utils.mel_filter_bank, WFE:95-103) with the first/last non-zero bin of each filter in mel_klo/khi,
