@@ -52,6 +52,9 @@ SIGNATURES = {
     "af3_lm_head_xent_scratch_bytes": (_sz, [_i, _i]),
     "af3_lm_head_xent": (_i, [_p, _p, _i, _p, _i, _i, _i, _i, _p, _i64, _p, _i, _p, _p, _p]),
     "af3_gemm_qkv_rope_fp8": (_i, [_p, _p, _i, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz]),
+    "af3_gemm_w4a16": (_i, [_p, _p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p, _p, _i, _p, _sz]),
+    "af3_gemm_qkv_rope_w4a16": (_i, [_p, _p, _i, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _i, _p, _p, _sz]),
+    "af3_dequant_w4a16": (_i, [_p, _p, _i, _p, _i, _p, _i, _i]),
 }
 
 

@@ -120,6 +120,28 @@ int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_s
                          0, workspace, workspace_bytes, &r);
 }
 
+int af3_gemm_w4a16(void* stream, const void* x, int ldx, const void* w_packed, int ldw, const void* w_scale, int ld_scale, void* out,
+                   int ldo, int n_tok, int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res, void* workspace,
+                   size_t workspace_bytes) {
+    if (flags & AF3_EPI_ROPE_INTERNAL) return af3::fail("af3_gemm_w4a16: use af3_gemm_qkv_rope_w4a16 for the RoPE epilogue");
+    return af3::gemm_w4a16(S(stream), B16(x), ldx, reinterpret_cast<const uint32_t*>(w_packed), ldw, B16(w_scale), ld_scale, out, ldo,
+                           n_tok, n_feat, K, flags, B16(bias), B16(resid), ld_res, workspace, workspace_bytes, nullptr);
+}
+
+int af3_gemm_qkv_rope_w4a16(void* stream, const void* x, int ldx, const void* w_packed, int ldw, const void* w_scale, int ld_scale,
+                            const void* bias, void* q_out, int ldo, int n_tok, int K, int H, int Hkv, int D, const float* rope_cs,
+                            void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace, size_t workspace_bytes) {
+    if (D != 128) return af3::fail("af3_gemm_qkv_rope_w4a16: head_dim must be 128");
+    af3::RopeEpilogue r{rope_cs, B16M(k_cache), B16M(v_cache), pos_dev, H, Hkv, Tmax};
+    return af3::gemm_w4a16(S(stream), B16(x), ldx, reinterpret_cast<const uint32_t*>(w_packed), ldw, B16(w_scale), ld_scale, q_out, ldo,
+                           n_tok, (H + 2 * Hkv) * D, K, AF3_EPI_BIAS | AF3_EPI_ROPE_INTERNAL, B16(bias), nullptr, 0, workspace,
+                           workspace_bytes, &r);
+}
+
+int af3_dequant_w4a16(void* stream, const void* w_packed, int ldw, const void* w_scale, int ld_scale, void* out, int rows, int K) {
+    return af3::dequant_w4a16(S(stream), reinterpret_cast<const uint32_t*>(w_packed), ldw, B16(w_scale), ld_scale, B16M(out), rows, K);
+}
+
 size_t af3_lm_head_xent_scratch_bytes(int n_tok, int V) { return af3::lm_head_xent_scratch_bytes(n_tok, V); }
 int af3_lm_head_xent(void* stream, const void* x, int ldx, const void* w, int ldw, int n_tok, int V, int K, const int64_t* labels,
                      int64_t ignore_index, float* logits_out, int ldo, float* token_nll, double* totals, void* scratch) {

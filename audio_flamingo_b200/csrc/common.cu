@@ -30,12 +30,13 @@ static PFN_encodeTiled get_encode() {
 }
 
 static int encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_b,
-                  const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+                  const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                  CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     PFN_encodeTiled fn = get_encode();
     if (!fn) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_b,
-                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         return fail("cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r) + " (rank " +
@@ -56,13 +57,14 @@ int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t cols, uint64_t row
 }
 
 int make_tmap_2d_u8(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch_bytes, uint32_t box_cols,
-                    uint32_t box_rows) {
+                    uint32_t box_rows, bool swizzle_64b) {
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("TMA base pointer must be 16-byte aligned");
     if (pitch_bytes % 16 != 0) return fail("TMA row pitch must be a multiple of 16 bytes");
     cuuint64_t dims[2] = {cols, rows};
     cuuint64_t strides[1] = {pitch_bytes};
     cuuint32_t box[2] = {box_cols, box_rows};
-    return encode(map, base, 2, dims, strides, box, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    return encode(map, base, 2, dims, strides, box, CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                  swizzle_64b ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t p1_elems,

@@ -34,9 +34,10 @@ int fail(const std::string& msg);  // records msg, returns a non-zero status
 // 2-D: dims (inner = cols, outer = rows), row pitch in elements.
 int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch_elems,
                  uint32_t box_cols, uint32_t box_rows);
-// The same for one-byte elements (e4m3): box inner extent 128 elements (128 B), pitch in bytes.
+// The same for one-byte elements (e4m3): box inner extent 128 elements (128 B), pitch in bytes.  swizzle_64b: 64-byte swizzle
+// for a 64-byte box inner extent (packed int4 weights, two nibbles per byte).
 int make_tmap_2d_u8(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t pitch_bytes, uint32_t box_cols,
-                    uint32_t box_rows);
+                    uint32_t box_rows, bool swizzle_64b = false);
 // 3-D: dims (d0 = cols, d1, d2) with element pitches p1, p2.
 int make_tmap_3d(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t p1_elems,
                  uint64_t p2_elems, uint32_t box0, uint32_t box1, uint32_t box2);

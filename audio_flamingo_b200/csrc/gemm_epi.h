@@ -28,6 +28,12 @@ int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, co
              void* out, int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res,
              void* workspace, size_t workspace_bytes, const RopeEpilogue* rope);
 int quant_fp8(cudaStream_t stream, const bf16* x, int ldx, uint8_t* q, float* scales, int rows, int K);
+// Group-wise int4 weights, bf16 activations (include/af3b200.h af3_gemm_w4a16 / af3_dequant_w4a16): w packed [rows, K/8]
+// int32 (pitch ldw words), w_scale bf16 [rows, K/128] (pitch ld_scale); few-token GEMM only (n_tok <= 64)
+int gemm_w4a16(cudaStream_t stream, const bf16* x, int ldx, const uint32_t* w, int ldw, const bf16* w_scale, int ld_scale, void* out,
+               int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, void* workspace,
+               size_t workspace_bytes, const RopeEpilogue* rope);
+int dequant_w4a16(cudaStream_t stream, const uint32_t* w, int ldw, const bf16* w_scale, int ld_scale, bf16* out, int rows, int K);
 // LM head with the cross-entropy statistics in its epilogue (include/af3b200.h af3_lm_head_xent)
 size_t lm_head_xent_scratch_bytes(int n_tok, int V);
 int lm_head_xent(cudaStream_t stream, const bf16* x, int ldx, const bf16* w, int ldw, int n_tok, int V, int K, const int64_t* labels,

@@ -84,6 +84,9 @@ struct GemmArgs {
     const float* sx;
     const float* sw;
     int ld_sw;
+    // W4A16 few-token kernel: one bf16 scale per weight row and 128-column group, [w_rows][ld_ws]
+    const bf16* ws_w4;
+    int ld_ws;
     // EPI_XENT (lm_head_xent): labels [n_tok] (shifted), one (max, sum exp) partial per (token, column tile) at
     // xent_part[tok * num_c_tiles + c], the label's bf16-rounded logit at xent_tgt[tok]
     const int64_t* labels;
@@ -239,10 +242,16 @@ constexpr int FP8_TOK_STAGES = 6;
 // ---- few-token (swap) mode
 constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups (wgmma; warps 0-3 also run the epilogue), warp 8: TMA producer
 
-template <int BN, int NA, int STAGES>
+// Weight operand of the few-token kernel: bf16, block-scaled e4m3 (gemm_fp8) or group-wise int4 (gemm_w4a16)
+enum WMode : int { WM_BF16 = 0, WM_FP8 = 1, WM_W4 = 2 };
+
+// W4: a stage holds 128 K -- per 128-row block 128 x 64 bytes of packed nibbles -- and the 128 matching bf16 activation
+// columns as two 128-byte swizzle atoms of BN rows
+template <int BN, int NA, int STAGES, bool W4 = false>
 struct GemmCfg {
-    static constexpr int R_BYTES = 128 * NA * BK * 2;
-    static constexpr int C_BYTES = BN * BK * 2;
+    static constexpr int R_BLOCK_BYTES = W4 ? 128 * 64 : 128 * BK * 2;  // one 128-row block of the row operand
+    static constexpr int R_BYTES = NA * R_BLOCK_BYTES;
+    static constexpr int C_BYTES = W4 ? 2 * BN * BK * 2 : BN * BK * 2;
     static constexpr int STAGE_BYTES = R_BYTES + C_BYTES;
     static constexpr int ACC_COLS = NA * BN;
     // the finished fp32 accumulator tile [128 rows][ACC_COLS], handed from the wgmma registers to the epilogue warps
@@ -838,18 +847,41 @@ gemm_fp8_tok_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     if (threadIdx.x == 0) trace_mark(a.trace, 3);
 }
 
+// ---- W4A16 weights (include/af3b200.h af3_gemm_w4a16): bits 4j .. 4j + 3 of word i of a packed row hold q[8i + j] + 8.
+// Byte b of a word (columns 2b, 2b + 1 of its 8) as the bf16x2 Wd = bf16(q * s): the two nibbles become the low mantissa
+// bits of 128.0 (0x4300 | u = 128 + u, exact), 136 = 128 + 8 is subtracted (exact), and one bf16 multiply by the group
+// scale rounds once, to nearest even -- what torch's q.to(bf16) * s gives.  sel = w4_sel(b).
+__device__ __forceinline__ uint32_t w4_sel(int b) { return b | (b << 4) | ((b + 4) << 8) | ((b + 4) << 12); }
+__device__ __forceinline__ uint32_t w4_pair(uint32_t word, uint32_t sel, __nv_bfloat162 s2) {
+    const uint32_t x = (__byte_perm(word, word >> 4, sel) & 0x000F000Fu) | 0x43004300u;  // byte b at bits 0-7, (word >> 4)'s at 16-23
+    __nv_bfloat162 h = *reinterpret_cast<const __nv_bfloat162*>(&x);
+    h = __hmul2(__hsub2(h, __floats2bfloat162_rn(136.f, 136.f)), s2);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+__device__ __forceinline__ __nv_bfloat162 w4_scale2(uint16_t bits) {
+    const uint32_t v = bits * 0x10001u;
+    return *reinterpret_cast<const __nv_bfloat162*>(&v);
+}
+
 // ============================================================================ few-token (swap) mode (n_tok <= 64)
 // EPI >= 0: epilogue flags fixed at compile time (no per-element branches, full ILP across the 32-column chunk);
 // EPI < 0: generic instantiation reading a.flags at run time (odd layouts / unusual flag mixes).
-// FP8: both operands e4m3 with block scales (gemm_fp8).  A stage then holds 128 K (one 128-byte swizzle row = one scale
+// WM_FP8: both operands e4m3 with block scales (gemm_fp8).  A stage then holds 128 K (one 128-byte swizzle row = one scale
 // group) in the same bytes as 64 bf16 K.  Each k-block is accumulated by m64n32k32 QGMMAs into its own registers and
 // promoted into the fp32 accumulator with sw (of the weight rows' 128-row block) x sx (of each token column), so the
 // tensor-core accumulation never spans two k-blocks.  The epilogue first rounds the result to bf16 (FP8Linear's output).
-template <int BN, int NA, int STAGES, int EPI, bool FP8 = false>
+// WM_W4: group-wise int4 weights, bf16 activations (gemm_w4a16).  A k-block is 128 K = one scale group: 64 bytes of packed
+// nibbles per weight row (64-byte swizzle) and the two 64-column activation atoms.  Each consumer thread converts its
+// nibbles straight into the register layout of the wgmma A fragment (Wd, rounded to bf16 as af3_dequant_w4a16 does) and
+// issues m64n32k16 with A from registers, in the k16 order of the bf16 kernel: unsplit, the result is that of
+// af3_gemm_bf16 on Wd bit for bit.
+template <int BN, int NA, int STAGES, int EPI, int WM = WM_BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_c, const GemmArgs a) {
-    using Cfg = GemmCfg<BN, NA, STAGES>;
-    constexpr int KB = FP8 ? 128 : BK;  // K elements per k-block (128 bytes of every row either way)
+    constexpr bool FP8 = WM == WM_FP8, W4 = WM == WM_W4;
+    using Cfg = GemmCfg<BN, NA, STAGES, W4>;
+    constexpr int KB = (FP8 || W4) ? 128 : BK;  // K elements per k-block
+    constexpr int KB_R = W4 ? 64 : KB;          // its extent in the row operand's tensor map (W4: bytes of packed nibbles)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     float* accbuf = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
@@ -894,6 +926,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                 }
             }
         }
+        if constexpr (W4) {
+            // the scale rows of the first work item's weight rows (contiguous: 128 rows x ld_ws bf16 per block), likewise
+            if (blockIdx.x < num_tiles) {
+                int r, c;
+                tile_coords(blockIdx.x / k_splits, a, r, c);
+#pragma unroll
+                for (int na = 0; na < NA; ++na) {
+                    const char* p = reinterpret_cast<const char*>(
+                        a.ws_w4 + static_cast<size_t>(a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128) * a.ld_ws);
+                    for (int o = lane * 128; o < 128 * a.ld_ws * 2; o += 32 * 128) prefetch_l2(p + o);
+                }
+            }
+        }
         if (lane == 0) {
             Ring<STAGES> ring;
             // The row operand is a WEIGHT matrix, independent of earlier kernels -> its first STAGES tiles are
@@ -910,7 +955,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         uint8_t* sR = smem + prefetched * Cfg::STAGE_BYTES;
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
-                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[prefetched], kb * KB,
+                            tma_load_2d(sR + na * Cfg::R_BLOCK_BYTES, &map_r, &full[prefetched], kb * KB_R,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
                 }
@@ -929,10 +974,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         mbar_arrive_expect_tx(&full[ring.stage], Cfg::STAGE_BYTES);
 #pragma unroll
                         for (int na = 0; na < NA; ++na)
-                            tma_load_2d(sR + na * 128 * BK * 2, &map_r, &full[ring.stage], kb * KB,
+                            tma_load_2d(sR + na * Cfg::R_BLOCK_BYTES, &map_r, &full[ring.stage], kb * KB_R,
                                         a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128);
                     }
                     tma_load_2d(sC, &map_c, &full[ring.stage], kb * KB, c * BN);
+                    if constexpr (W4) tma_load_2d(sC + BN * BK * 2, &map_c, &full[ring.stage], kb * KB + BK, c * BN);
                     ring.next();
                 }
             }
@@ -1020,6 +1066,76 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                                 accr[na][i] = fmaf(kacc[na][i], sw[na] * sx[j], accr[na][i]);
                             }
                     }
+                } else if constexpr (W4) {
+                    int r, c;
+                    tile_coords(t / k_splits, a, r, c);
+                    // this thread's A-fragment rows lrow and lrow + 8 of every 128-row block, and the byte of each packed word
+                    // it converts: columns 2 (tw % 4) and + 1 of every 8 (the fragment's columns c, c + 1 and c + 8, c + 9)
+                    const int lrow = wg * 64 + frag_row(tw, 0);
+                    const uint32_t sel = w4_sel(tw & 3);
+                    const uint16_t* scp[NA][2];
+#pragma unroll
+                    for (int na = 0; na < NA; ++na)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            scp[na][h] = reinterpret_cast<const uint16_t*>(a.ws_w4) +
+                                         static_cast<size_t>((a.swiglu_up_row0 ? na * a.swiglu_up_row0 + r * 128 : (r * NA + na) * 128) + lrow + 8 * h) * a.ld_ws;
+                    const int kb_end = kb_lo(sp + 1);
+                    // group scales two k-blocks ahead of their use: the L2 round trip hides behind two k-blocks of work
+                    uint16_t sc0[NA][2], sc1[NA][2];
+                    auto ld_sc = [&](uint16_t (&d)[NA][2], int kb) {
+#pragma unroll
+                        for (int na = 0; na < NA; ++na)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) d[na][h] = kb < kb_end ? __ldg(scp[na][h] + kb) : uint16_t(0);
+                    };
+                    ld_sc(sc0, kb_lo(sp));
+                    ld_sc(sc1, kb_lo(sp) + 1);
+                    for (int kb = kb_lo(sp); kb < kb_end; ++kb) {
+                        uint16_t sc2[NA][2];
+                        ld_sc(sc2, kb + 2);
+                        mbar_wait(&full[ring.stage], ring.phase);
+                        const uint8_t* sR = smem + ring.stage * Cfg::STAGE_BYTES;
+                        const uint32_t sC = smem_u32(sR) + Cfg::R_BYTES;
+                        uint32_t af[NA][8][4];  // A fragments of the k-block's eight k16 steps
+#pragma unroll
+                        for (int na = 0; na < NA; ++na)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int row = lrow + 8 * h;
+                                const uint8_t* rp = sR + na * Cfg::R_BLOCK_BYTES + row * 64;
+                                const __nv_bfloat162 s2 = w4_scale2(sc0[na][h]);
+#pragma unroll
+                                for (int j = 0; j < 4; ++j) {
+                                    // words 4j .. 4j + 3 = k16 steps 2j, 2j + 1; 16-byte chunk j sits at j ^ ((row / 2) % 4) (64-byte swizzle)
+                                    const uint4 w = *reinterpret_cast<const uint4*>(rp + ((j ^ ((row >> 1) & 3)) << 4));
+                                    af[na][2 * j][h] = w4_pair(w.x, sel, s2);
+                                    af[na][2 * j][2 + h] = w4_pair(w.y, sel, s2);
+                                    af[na][2 * j + 1][h] = w4_pair(w.z, sel, s2);
+                                    af[na][2 * j + 1][2 + h] = w4_pair(w.w, sel, s2);
+                                }
+                            }
+                        fence();
+                        wgmma_fence();
+#pragma unroll
+                        for (int s = 0; s < 8; ++s) {
+                            const uint64_t bdesc = make_smem_desc_sw128(sC + (s >> 2) * (BN * BK * 2) + (s & 3) * 32, 0, 1024);
+#pragma unroll
+                            for (int na = 0; na < NA; ++na) wgmma_m64n32_rs<0>(accr[na], af[na][s], bdesc, 1);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();  // the fragments' registers are rewritten by the next k-block
+                        fence();
+                        if (lane == 0) mbar_arrive(&empty[ring.stage]);
+                        ring.next();
+#pragma unroll
+                        for (int na = 0; na < NA; ++na)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                sc0[na][h] = sc1[na][h];
+                                sc1[na][h] = sc2[na][h];
+                            }
+                    }
                 } else {
                     const int held = ring_mma(ring, full, empty, kb_lo(sp + 1) - kb_lo(sp), [&](int stage) {
                         const uint32_t sR = smem_u32(smem + stage * Cfg::STAGE_BYTES);
@@ -1051,9 +1167,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
             // few-token mode with a fused residual: this thread's residual vectors of the transposed epilogue (token et / 4,
             // features (et % 4) * 32 ...) do not depend on this GEMM -- request them now, they arrive while the weights stream
             // (the epilogue otherwise exposes one more L2 round trip in the split-K tail)
+            // (not in the W4 kernel: holding these 16 registers through the split-K reduction makes it spill)
+            constexpr bool RV_PRE = NA == 1 && !W4;
             [[maybe_unused]] uint4 rv_pre[4];
             [[maybe_unused]] bool rv_ok = false;
-            if constexpr (NA == 1) {
+            if constexpr (RV_PRE) {
                 if ((flags & EPI_RESID) && !(flags & EPI_F32OUT) && (a.ldo & 7) == 0 && (a.ld_res & 7) == 0 && a.res_period == 0) {
                     const int et = threadIdx.x;
                     const int tok = c * BN + (et >> 2);
@@ -1195,7 +1313,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ C
                         bf16* op = reinterpret_cast<bf16*>(a.out) + static_cast<size_t>(tok) * a.ldo + f0;
                         uint4 rv[4];
                         if (flags & EPI_RESID) {
-                            if constexpr (NA == 1) {
+                            if constexpr (RV_PRE) {
                                 if (rv_ok) {   // requested before the accumulator wait (same token / features)
 #pragma unroll
                                     for (int g4 = 0; g4 < 4; ++g4) rv[g4] = rv_pre[g4];
@@ -1526,12 +1644,12 @@ int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, co
     if (int e = make_tmap_2d_u8(&mw, w, K, w_rows, ldw, 128, 128)) return e;
     if (int e = make_tmap_2d_u8(&mx, x, K, n_tok, ldx, 128, BN)) return e;
     if (swiglu)  // ring depth as in gemm_bf16: as many stages as fit beside the accumulator tile
-        return launch_gemm<gemm_kernel<BN, 2, 5, EPI_SWIGLU, true>, GemmCfg<BN, 2, 5>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
+        return launch_gemm<gemm_kernel<BN, 2, 5, EPI_SWIGLU, WM_FP8>, GemmCfg<BN, 2, 5>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
     choose_k_splits(a, K / 128, workspace, workspace_bytes);
     switch (flags) {
 #define AF3_EPI_CASE(F) \
     case (F):           \
-        return launch_gemm<gemm_kernel<BN, 1, 10, (F), true>, GemmCfg<BN, 1, 10>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
+        return launch_gemm<gemm_kernel<BN, 1, 10, (F), WM_FP8>, GemmCfg<BN, 1, 10>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
         AF3_EPI_CASE(0)
         AF3_EPI_CASE(EPI_BIAS)
         AF3_EPI_CASE(EPI_RESID)
@@ -1540,6 +1658,110 @@ int gemm_fp8(cudaStream_t stream, const uint8_t* x, int ldx, const float* sx, co
         default:
             return fail("gemm_fp8: unsupported epilogue");
     }
+}
+
+// ============================================================================ W4A16 (include/af3b200.h af3_gemm_w4a16)
+// Ring depth as in gemm_bf16, as many stages as fit beside the accumulator tile: 12 x 16 KB (NA = 1), 7 x 24 KB (NA = 2).
+constexpr int W4_STAGES = 12, W4_SWIGLU_STAGES = 7;
+
+int gemm_w4a16(cudaStream_t stream, const bf16* x, int ldx, const uint32_t* w, int ldw, const bf16* w_scale, int ld_scale, void* out,
+               int ldo, int n_tok, int n_feat, int K, int flags, const bf16* bias, const bf16* resid, int ld_res, void* workspace,
+               size_t workspace_bytes, const RopeEpilogue* rope) {
+    AF3_REQUIRE(n_tok > 0 && n_feat > 0 && K > 0, "gemm_w4a16: empty problem");
+    AF3_REQUIRE(n_tok <= 64, "gemm_w4a16: n_tok must be at most 64 (the few-token kernel); above that, af3_dequant_w4a16 and af3_gemm_bf16");
+    AF3_REQUIRE(K % 128 == 0 && n_feat % 128 == 0, "gemm_w4a16: K and n_feat must be multiples of 128 (the scale groups)");
+    AF3_REQUIRE(ldx % 8 == 0 && ldx >= K, "gemm_w4a16: ldx must be a multiple of 8 and at least K");
+    AF3_REQUIRE(ldw % 4 == 0 && ldw >= K / 8, "gemm_w4a16: ldw (int32 words) must be a multiple of 4 and at least K / 8");
+    AF3_REQUIRE(w_scale && ld_scale >= K / 128, "gemm_w4a16: w_scale required, ld_scale >= K / 128");
+    AF3_REQUIRE(!(flags & EPI_BIAS) || bias, "gemm_w4a16: bias flag without pointer");
+    AF3_REQUIRE(!(flags & EPI_RESID) || resid, "gemm_w4a16: residual flag without pointer");
+    const bool swiglu = flags & EPI_SWIGLU;
+    AF3_REQUIRE(!swiglu || (flags & EPI_SWIGLU_CONCAT), "gemm_w4a16: SwiGLU needs the [gate; up] layout (AF3_EPI_SWIGLU_CONCAT)");
+    flags &= ~EPI_SWIGLU_CONCAT;
+    AF3_REQUIRE(flags == 0 || flags == EPI_BIAS || flags == EPI_RESID || flags == EPI_SWIGLU || flags == (EPI_BIAS | EPI_ROPE),
+                "gemm_w4a16: supported epilogues are none, bias, residual, SwiGLU and bias + RoPE");
+    const int w_rows = swiglu ? 2 * n_feat : n_feat;
+    GemmArgs a{};
+    a.K = K;
+    a.n_tok = n_tok;
+    a.n_feat = n_feat;
+    a.out = out;
+    a.ldo = ldo;
+    a.bias = bias;
+    a.resid = resid;
+    a.ld_res = ld_res;
+    a.flags = flags;
+    a.swiglu_up_row0 = swiglu ? n_feat : 0;
+    a.ws_w4 = w_scale;
+    a.ld_ws = ld_scale;
+    a.k_splits = 1;
+    a.trace = trace_next_slot();
+    if (flags & EPI_ROPE) {
+        AF3_REQUIRE(rope && rope->cs && rope->k_cache && rope->v_cache && rope->pos, "gemm_w4a16: EPI_ROPE needs the rope arguments");
+        AF3_REQUIRE(n_feat == (rope->H + 2 * rope->Hkv) * 128 && (ldo % 8) == 0,
+                    "gemm_w4a16: EPI_ROPE is the few-token fused q/k/v projection with head_dim 128");
+        a.rope_cs = reinterpret_cast<const float2*>(rope->cs);
+        a.k_cache = rope->k_cache;
+        a.v_cache = rope->v_cache;
+        a.rope_pos = rope->pos;
+        a.rope_H = rope->H;
+        a.rope_Hkv = rope->Hkv;
+        a.rope_Tmax = rope->Tmax;
+    }
+    constexpr int BN = 32;
+    a.num_c_tiles = ceil_div(n_tok, BN);
+    a.group_r = 1;
+    CUtensorMap mw, mx;
+    if (int e = make_tmap_2d_u8(&mw, w, K / 2, w_rows, static_cast<uint64_t>(ldw) * 4, 64, 128, true)) return e;
+    if (int e = make_tmap_2d(&mx, x, K, n_tok, ldx, BK, BN)) return e;
+    if (swiglu) {
+        a.num_r_tiles = w_rows / 256;
+        return launch_gemm<gemm_kernel<BN, 2, W4_SWIGLU_STAGES, EPI_SWIGLU, WM_W4>, GemmCfg<BN, 2, W4_SWIGLU_STAGES, true>::SMEM_BYTES,
+                           GEMM_THREADS>(a, stream, mw, mx);
+    }
+    a.num_r_tiles = w_rows / 128;
+    choose_k_splits(a, K / 128, workspace, workspace_bytes);
+    switch (flags) {
+#define AF3_EPI_CASE(F) \
+    case (F):           \
+        return launch_gemm<gemm_kernel<BN, 1, W4_STAGES, (F), WM_W4>, GemmCfg<BN, 1, W4_STAGES, true>::SMEM_BYTES, GEMM_THREADS>(a, stream, mw, mx);
+        AF3_EPI_CASE(0)
+        AF3_EPI_CASE(EPI_BIAS)
+        AF3_EPI_CASE(EPI_RESID)
+        AF3_EPI_CASE(EPI_BIAS | EPI_ROPE)
+#undef AF3_EPI_CASE
+        default:
+            return fail("gemm_w4a16: unsupported epilogue");
+    }
+}
+
+// Wd [rows, K] (pitch K) from the packed words: one word (8 values, one 16-byte store) per thread and loop step, converted by
+// the few-token kernel's w4_pair, so both paths compute with the same bf16 values.
+__global__ void __launch_bounds__(256)
+dequant_w4a16_kernel(const uint32_t* __restrict__ w, int ldw, const uint16_t* __restrict__ s, int ld_s, bf16* __restrict__ out, int rows, int K) {
+    const int wpr = K / 8;
+    const long long n = static_cast<long long>(rows) * wpr;
+    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * 256) {
+        const int row = static_cast<int>(i / wpr), wi = static_cast<int>(i - static_cast<long long>(row) * wpr);
+        const uint32_t word = __ldg(w + static_cast<size_t>(row) * ldw + wi);
+        const __nv_bfloat162 s2 = w4_scale2(__ldg(s + static_cast<size_t>(row) * ld_s + wi / 16));
+        const uint4 o = make_uint4(w4_pair(word, w4_sel(0), s2), w4_pair(word, w4_sel(1), s2), w4_pair(word, w4_sel(2), s2),
+                                   w4_pair(word, w4_sel(3), s2));
+        *reinterpret_cast<uint4*>(out + static_cast<size_t>(row) * K + 8 * wi) = o;
+    }
+}
+
+int dequant_w4a16(cudaStream_t stream, const uint32_t* w, int ldw, const bf16* w_scale, int ld_scale, bf16* out, int rows, int K) {
+    AF3_REQUIRE(rows > 0 && K > 0 && K % 128 == 0, "dequant_w4a16: rows > 0 and K a multiple of 128 (the scale groups) required");
+    AF3_REQUIRE(w && w_scale && out, "dequant_w4a16: null pointer");
+    AF3_REQUIRE(ldw >= K / 8 && ld_scale >= K / 128, "dequant_w4a16: ldw >= K / 8 and ld_scale >= K / 128 required");
+    AF3_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "dequant_w4a16: out must be 16-byte aligned");
+    const long long n = static_cast<long long>(rows) * (K / 8);
+    const long long blocks = (n + 255) / 256;
+    const int grid = static_cast<int>(blocks < 16ll * sm_count() ? blocks : 16ll * sm_count());
+    dequant_w4a16_kernel<<<grid, 256, 0, stream>>>(w, ldw, reinterpret_cast<const uint16_t*>(w_scale), ld_scale, out, rows, K);
+    AF3_CHECK_LAUNCH();
+    return 0;
 }
 
 // ============================================================================ LM head + cross-entropy (lm_head_xent)

@@ -136,6 +136,32 @@ def dequantize_fp8_blocks(q, scale_inv):
     return (q.to(torch.float32).reshape(rows // 128, 128, cols // 128, 128) * scale_inv[:, None, :, None]).reshape(rows, cols)
 
 
+# W4A16 weights (include/af3b200.h af3_gemm_w4a16): symmetric int4, one bf16 scale per row and 128 columns, 8 values per int32
+W4_GROUP = 128
+
+
+def quantize_w4a16(w):
+    """w [rows, cols] (cols % 128 == 0) -> (weight_packed int32 [rows, cols / 8], weight_scale bf16 [rows, cols / 128]).
+    s = bf16(amax / 7.5) per group (1 for an all-zero group), q = clamp(round_half_even(w / s), -8, 7) in fp32; bits 4j .. 4j+3
+    of word i hold q[8i + j] + 8.  Load-time only; runs wherever w lives."""
+    rows, cols = w.shape
+    g = w.to(torch.float32).reshape(rows, cols // W4_GROUP, W4_GROUP)
+    amax = g.abs().amax(-1)
+    s = torch.where(amax > 0, amax / torch.full_like(amax, 7.5), torch.ones_like(amax)).to(bf16)
+    q = torch.clamp(torch.round(g / s.to(torch.float32)[..., None]), -8, 7).to(torch.int32) + 8
+    nib = q.to(torch.int64).reshape(rows, cols // 8, 8) << (4 * torch.arange(8, device=w.device, dtype=torch.int64))
+    v = nib.sum(-1)  # the word as an unsigned 32-bit value; stored as the int32 with the same bits
+    return torch.where(v >= (1 << 31), v - (1 << 32), v).to(torch.int32), s
+
+
+def dequantize_w4a16(packed, scale):
+    """Wd = bf16(q * s) [rows, cols] from weight_packed int32 [rows, cols / 8] and weight_scale bf16 [rows, cols / 128]."""
+    rows, words = packed.shape
+    q = (packed.to(torch.int64)[..., None] >> (4 * torch.arange(8, device=packed.device, dtype=torch.int64))) & 15
+    q = (q - 8).reshape(rows, words * 8)
+    return q.to(bf16) * scale.repeat_interleave(W4_GROUP, dim=1)
+
+
 def _is_decoder_projection(key):
     """'language_model.model.layers.<i>.<proj>' for the seven FP8 projections of a decoder layer"""
     return key.startswith("language_model.model.layers.") and any(key.endswith("." + p) for p in DECODER_PROJECTIONS)
@@ -409,6 +435,45 @@ class _Fp8Projections:
         ops.linear_fp8(ops.quant_fp8(g), *self.wdown, resid=h, out=h)
 
 
+class _W4A16Projections:
+    """The same four GEMMs on group-wise int4 weights, each a (weight_packed, weight_scale) pair.  Up to 64 tokens the
+    W4A16 few-token GEMMs run; above that (prefill, decode with more than 64 sequences) af3_dequant_w4a16 writes the
+    projection's Wd into the layer stack's one bf16 scratch and the bf16 GEMM runs on it, so those results are the bf16
+    model's on Wd bit for bit."""
+
+    def __init__(self, lm, wqkv, bqkv, wo, wgu, wdown):
+        self.lm, self.wqkv, self.bqkv, self.wo, self.wgu, self.wdown = lm, wqkv, bqkv, wo, wgu, wdown
+
+    def _wd(self, w):
+        return ops.dequant_w4a16(*w, out=self.lm._w4_scratch)
+
+    def qkv(self, y):
+        if y.shape[0] <= 64:
+            return ops.linear_w4a16(y, *self.wqkv, self.bqkv)
+        return ops.linear(y, self._wd(self.wqkv), self.bqkv)
+
+    def qkv_rope(self, y, kc, vc, rope_cs, pos_dev):
+        lm = self.lm
+        return ops.qkv_rope_linear_w4a16(y, *self.wqkv, self.bqkv, kc, vc, H=lm.H, Hkv=lm.Hkv, D=lm.D, rope_cs=rope_cs, pos_dev=pos_dev)
+
+    def o(self, a, h):
+        if a.shape[0] <= 64:
+            ops.linear_w4a16(a, *self.wo, resid=h, out=h)
+        else:
+            ops.linear(a, self._wd(self.wo), resid=h, out=h)
+
+    def gate_up(self, y):
+        if y.shape[0] <= 64:
+            return ops.swiglu_linear_w4a16(y, *self.wgu, self.lm.inter)
+        return ops.swiglu_linear(y, self._wd(self.wgu), self.lm.inter, concat=True)
+
+    def down(self, g, h):
+        if g.shape[0] <= 64:
+            ops.linear_w4a16(g, *self.wdown, resid=h, out=h)
+        else:
+            ops.linear(g, self._wd(self.wdown), resid=h, out=h)
+
+
 class Qwen2ForCausalLM(nn.Module):
     """Decoder ([O] Q2M:332-487) on sm_90a kernels: RMSNorm, fused QKV GEMM (+bias), RoPE + in-place KV append,
     wgmma causal GQA attention (prefill) / split-KV decode attention, o GEMM (+residual), fused SwiGLU GEMM,
@@ -430,7 +495,9 @@ class Qwen2ForCausalLM(nn.Module):
             raise AF3Error("only default RoPE is implemented")
         self.model = _Qwen2Model(tc)
         self.lm_head = nn.Linear(self.hid, self.vocab, bias=False)
-        self.quantization = None  # "fp8": the decoder projections hold e4m3 weights + weight_scale_inv (load_reference_state_dict)
+        self.quantization = None  # "fp8": the decoder projections hold e4m3 weights + weight_scale_inv (load_reference_state_dict);
+        # "w4a16": they hold weight_packed + weight_scale instead of weight
+        self._w4_scratch = None
         self._packed = None
         self._proj = None
         self._inv_freq = None
@@ -446,6 +513,8 @@ class Qwen2ForCausalLM(nn.Module):
         self._swiglu_concat = self.inter % 128 == 0
         if self.quantization == "fp8":
             return self._pack_fp8()
+        if self.quantization == "w4a16":
+            return self._pack_w4a16()
         for l in self.model.layers:
             a, m = l.self_attn, l.mlp
             wqkv = torch.cat([a.q_proj.weight.detach(), a.k_proj.weight.detach(), a.v_proj.weight.detach()], 0).contiguous()
@@ -483,6 +552,32 @@ class Qwen2ForCausalLM(nn.Module):
             P.append((wqkv, bqkv, wgu))
             proj.append(_Fp8Projections(self, (wqkv, sqkv), bqkv, (a.o_proj.weight, a.o_proj.weight_scale_inv), (wgu, sgu),
                                         (m.down_proj.weight, m.down_proj.weight_scale_inv)))
+        self._packed, self._proj = P, proj
+        self._set_inv_freq()
+
+    def _pack_w4a16(self):
+        """W4A16 counterpart of pack_weights: one fused [q; k; v] and one [gate; up] packed matrix per layer with their scale
+        grids (packing is per row, so stacking rows is exact); the projections' weight_packed / weight_scale become row views
+        of them.  Also allocates the bf16 scratch that the GEMMs of more than 64 tokens dequantize into, sized for the largest
+        projection ([gate; up]: 272 MB at 7B)."""
+        P, proj = [], []
+        HD, KD = self.H * self.D, self.Hkv * self.D
+        for l in self.model.layers:
+            a, m = l.self_attn, l.mlp
+            wqkv = torch.cat([a.q_proj.weight_packed, a.k_proj.weight_packed, a.v_proj.weight_packed], 0).contiguous()
+            sqkv = torch.cat([a.q_proj.weight_scale, a.k_proj.weight_scale, a.v_proj.weight_scale], 0).contiguous()
+            bqkv = torch.cat([a.q_proj.bias.detach(), a.k_proj.bias.detach(), a.v_proj.bias.detach()], 0).contiguous()
+            wgu = torch.cat([m.gate_proj.weight_packed, m.up_proj.weight_packed], 0).contiguous()
+            sgu = torch.cat([m.gate_proj.weight_scale, m.up_proj.weight_scale], 0).contiguous()
+            for mod, w, sc, r0, r1 in ((a.q_proj, wqkv, sqkv, 0, HD), (a.k_proj, wqkv, sqkv, HD, HD + KD), (a.v_proj, wqkv, sqkv, HD + KD, HD + 2 * KD),
+                                       (m.gate_proj, wgu, sgu, 0, self.inter), (m.up_proj, wgu, sgu, self.inter, 2 * self.inter)):
+                mod.weight_packed, mod.weight_scale = w[r0:r1], sc[r0:r1]
+            a.q_proj.bias.data, a.k_proj.bias.data, a.v_proj.bias.data = bqkv[:HD], bqkv[HD:HD + KD], bqkv[HD + KD:]
+            P.append((wqkv, bqkv, wgu))
+            proj.append(_W4A16Projections(self, (wqkv, sqkv), bqkv, (a.o_proj.weight_packed, a.o_proj.weight_scale), (wgu, sgu),
+                                          (m.down_proj.weight_packed, m.down_proj.weight_scale)))
+        n = max(w.shape[0] * w.shape[1] * 8 for pj in proj for w, _ in (pj.wqkv, pj.wo, pj.wgu, pj.wdown))
+        self._w4_scratch = torch.empty((n,), device=self.lm_head.weight.device, dtype=bf16)
         self._packed, self._proj = P, proj
         self._set_inv_freq()
 
@@ -651,7 +746,7 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
     # ---- construction from the reference model / a reference state_dict
     @classmethod
     def from_reference(cls, ref_model, device="cuda", quantization=None):
-        """Build from an instantiated reference model (weights are copied, cast to bf16).  quantization="fp8": see
+        """Build from an instantiated reference model (weights are copied, cast to bf16).  quantization="fp8" or "w4a16": see
         load_reference_state_dict."""
         m = cls(ref_model.config)
         m.load_reference_state_dict(ref_model.state_dict(), device=device, quantization=quantization)
@@ -673,28 +768,61 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
 
         The state_dict may already be in that layout (`<name>.weight` float8_e4m3fn plus `<name>.weight_scale_inv`, what
         state_dict() of an FP8 model returns).  Its decoder projections are then used as they are, and the model is FP8
-        whatever `quantization` says.  Any other Linear stored that way is dequantized once to bf16."""
-        if quantization not in (None, "fp8"):
-            raise AF3Error(f"quantization must be None or 'fp8', got {quantization!r}")
+        whatever `quantization` says.  Any other Linear stored that way is dequantized once to bf16.
+
+        quantization="w4a16" stores the same seven projections as group-wise int4 (include/af3b200.h af3_gemm_w4a16): one
+        bf16 scale per row and 128 input columns, round to nearest, packed 8 values per int32.  The projection modules then
+        carry `weight_packed` and `weight_scale` instead of `weight`, and state_dict() returns those keys; a state_dict that
+        carries them for the decoder projections loads as W4A16 whatever `quantization` says (weights from another quantizer
+        in this layout load as they are).  Decode with up to 64 sequences runs the int4 GEMMs; larger token counts run the
+        bf16 GEMMs on the dequantized projection."""
+        if quantization not in (None, "fp8", "w4a16"):
+            raise AF3Error(f"quantization must be None, 'fp8' or 'w4a16', got {quantization!r}")
         scaled = {k[: -len(".weight_scale_inv")] for k in sd if k.endswith(".weight_scale_inv")}
+        packed = {k[: -len(".weight_packed")] for k in sd if k.endswith(".weight_packed")}
+        for base in sorted(packed):
+            if base + ".weight_scale" not in sd:
+                raise AF3Error(f"{base}.weight_packed without {base}.weight_scale")
         if any(_is_decoder_projection(k) for k in scaled):
             quantization = "fp8"
+        if any(_is_decoder_projection(k) for k in packed):
+            quantization = "w4a16"
         lm = self.language_model
-        for name in DECODER_PROJECTIONS:  # back to the plain bf16 module tree (a previous FP8 load added the scales)
-            for l in lm.model.layers:
-                mod = l.get_submodule(name)
-                if "weight_scale_inv" in mod._buffers:
-                    del mod._buffers["weight_scale_inv"]
-        if quantization == "fp8":
+        if quantization is not None:
             sizes = {"hidden_size": lm.hid, "q size": lm.H * lm.D, "k/v size": lm.Hkv * lm.D, "intermediate_size": lm.inter}
             bad = {k: v for k, v in sizes.items() if v % 128}
             if bad:
-                raise AF3Error(f"fp8 quantization needs multiples of 128 (the 128 x 128 scale blocks); got {bad}")
+                what = "the 128 x 128 scale blocks" if quantization == "fp8" else "the 128-column scale groups"
+                raise AF3Error(f"{quantization} quantization needs multiples of 128 ({what}); got {bad}")
+        for name in DECODER_PROJECTIONS:  # the module tree of this load: a previous FP8 / W4A16 load changed the projections
+            for l in lm.model.layers:
+                mod = l.get_submodule(name)
+                mod._buffers.pop("weight_scale_inv", None)
+                N, K = mod.out_features, mod.in_features
+                if quantization == "w4a16":
+                    mod._parameters.pop("weight", None)
+                    mod.register_buffer("weight_packed", torch.empty((N, K // 8), dtype=torch.int32, device="meta"))
+                    mod.register_buffer("weight_scale", torch.empty((N, K // W4_GROUP), dtype=bf16, device="meta"))
+                elif "weight_packed" in mod._buffers:
+                    del mod._buffers["weight_packed"], mod._buffers["weight_scale"]
+                    mod.weight = nn.Parameter(torch.empty((N, K), device="meta"))
         self.to_empty(device=device)
         self.to(bf16)
         own = self.state_dict()
-        missing = [k for k in own if k not in sd]
-        unexpected = [k for k in sd if k not in own and not (k.endswith(".weight_scale_inv") and k[: -len("_scale_inv")] in own)]
+        w4_own = {k[: -len(".weight_packed")] for k in own if k.endswith(".weight_packed")}
+
+        def present(k):  # a W4A16 projection may come as weight_packed + weight_scale or as a plain weight
+            for sfx in (".weight_packed", ".weight_scale"):
+                if k.endswith(sfx) and k[: -len(sfx)] in w4_own:
+                    return k[: -len(sfx)] in packed or k[: -len(sfx)] + ".weight" in sd
+            return k in sd
+
+        def expected(k):
+            if k in own or (k.endswith(".weight_scale_inv") and k[: -len("_scale_inv")] in own):
+                return True
+            return k.endswith(".weight") and k[: -len(".weight")] in w4_own
+        missing = [k for k in own if not present(k)]
+        unexpected = [k for k in sd if not expected(k)]
         if missing or unexpected:
             raise AF3Error(f"state_dict mismatch: missing {missing[:4]}..., unexpected {unexpected[:4]}...")
 
@@ -721,6 +849,17 @@ class AudioFlamingo3ForConditionalGeneration(nn.Module):
                         q, s = quantize_fp8_blocks(sd[k].to(device=v.device, dtype=bf16))
                     fp8_params[base] = (q.contiguous(), s.contiguous())
                     continue
+                if k.endswith(".weight_packed") and k[: -len(".weight_packed")] in w4_own:
+                    base = k[: -len(".weight_packed")]
+                    if base in packed:
+                        q, s = sd[k], sd[base + ".weight_scale"]
+                    else:
+                        q, s = quantize_w4a16(sd[base + ".weight"].to(device=v.device, dtype=bf16))
+                    v.copy_(q.to(device=v.device, dtype=torch.int32))
+                    own[base + ".weight_scale"].copy_(s.to(device=v.device, dtype=bf16))
+                    continue
+                if k.endswith(".weight_scale") and k[: -len(".weight_scale")] in w4_own:
+                    continue  # with its weight_packed
                 v.copy_(bf16_value(k).to(device=v.device, dtype=bf16))
             for base, (q, s) in fp8_params.items():
                 mod = self.get_submodule(base)

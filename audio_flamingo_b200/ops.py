@@ -263,6 +263,110 @@ def qkv_rope_linear_fp8(xq, w, w_scale_inv, bias, k_cache, v_cache, *, H, Hkv, D
     return out
 
 
+# ----------------------------------------------------------------------------------------------- W4A16 decoder projections
+def _w4_operands(x, w_packed, w_scale, rows_per_feat=1):
+    _req(x, bf16, "x"), _req(w_packed, torch.int32, "w_packed"), _req(w_scale, bf16, "w_scale")
+    n_tok, K = x.shape
+    N = w_packed.shape[0]
+    if K % 128 or N % (128 * rows_per_feat) or tuple(w_packed.shape) != (N, K // 8) or tuple(w_scale.shape) != (N, K // 128):
+        raise _lib.AF3Error(f"w4a16 GEMM: shapes x {tuple(x.shape)}, w_packed {tuple(w_packed.shape)}, w_scale {tuple(w_scale.shape)} "
+                            "do not match (w_packed [N, K / 8], w_scale [N, K / 128], K and N multiples of 128)")
+    if n_tok > 64:
+        raise _lib.AF3Error(f"w4a16 GEMM: at most 64 tokens, got {n_tok} (dequant_w4a16 + linear above that)")
+    return n_tok, K
+
+
+def linear_w4a16(x, w_packed, w_scale, bias=None, *, resid=None, out=None):
+    """out = epi(x @ Wd.T) with W4A16 weights (include/af3b200.h af3_gemm_w4a16), n_tok <= 64: x bf16 [n_tok, K], w_packed
+    int32 [n_feat, K / 8], w_scale bf16 [n_feat, K / 128]; bias, or resid (out may be resid)."""
+    lib = _lib.load()
+    n_tok, K = _w4_operands(x, w_packed, w_scale)
+    n_feat = w_packed.shape[0]
+    flags = 0
+    if bias is not None:
+        _req(bias, bf16, "bias")
+        flags |= EPI_BIAS
+    if resid is not None:
+        _req(resid, bf16, "resid")
+        flags |= EPI_RESID
+    if out is None:
+        out = torch.empty((n_tok, n_feat), device=x.device, dtype=bf16)
+    ws = gemm_workspace(x.device)
+    with _Timed(("gemm_w4a16", n_tok, n_feat, K, flags)):
+        check(
+            lib.af3_gemm_w4a16(stream_ptr(), ptr(x), x.stride(0), ptr(w_packed), w_packed.stride(0), ptr(w_scale), w_scale.stride(0),
+                               ptr(out), out.stride(0), n_tok, n_feat, K, flags, ptr(bias), ptr(resid),
+                               resid.stride(0) if resid is not None else 0, ptr(ws), ws.numel()),
+            "af3_gemm_w4a16",
+        )
+    _count(1)
+    return out
+
+
+def swiglu_linear_w4a16(x, w_packed, w_scale, n_feat, out=None):
+    """out = silu(x @ gate.T) * (x @ up.T) with W4A16 weights, n_tok <= 64: w_packed / w_scale hold the [gate; up]
+    concatenation ([2 n_feat, K / 8] and [2 n_feat, K / 128])."""
+    lib = _lib.load()
+    n_tok, K = _w4_operands(x, w_packed, w_scale, rows_per_feat=2)
+    if w_packed.shape[0] != 2 * n_feat:
+        raise _lib.AF3Error("swiglu_linear_w4a16: w_packed must hold 2 * n_feat rows")
+    if out is None:
+        out = torch.empty((n_tok, n_feat), device=x.device, dtype=bf16)
+    with _Timed(("gemm_w4a16", n_tok, n_feat, K, EPI_SWIGLU)):
+        check(
+            lib.af3_gemm_w4a16(stream_ptr(), ptr(x), x.stride(0), ptr(w_packed), w_packed.stride(0), ptr(w_scale), w_scale.stride(0),
+                               ptr(out), out.stride(0), n_tok, n_feat, K, EPI_SWIGLU | EPI_SWIGLU_CONCAT, None, None, 0, None, 0),
+            "af3_gemm_w4a16(swiglu)",
+        )
+    _count(1)
+    return out
+
+
+def qkv_rope_linear_w4a16(x, w_packed, w_scale, bias, k_cache, v_cache, *, H, Hkv, D, rope_cs, pos_dev, out=None):
+    """W4A16 counterpart of qkv_rope_linear (decode step, n_tok <= 64): returns the [n_tok, (H+2Hkv)*D] buffer whose first
+    H*D columns hold the rotated queries; rotated keys and the values go straight into the caches."""
+    lib = _lib.load()
+    n_tok, K = _w4_operands(x, w_packed, w_scale)
+    _req(bias, bf16, "bias")
+    if w_packed.shape[0] != (H + 2 * Hkv) * D:
+        raise _lib.AF3Error("qkv_rope_linear_w4a16: w_packed must hold (H + 2 Hkv) * D rows")
+    if out is None:
+        out = torch.empty((n_tok, (H + 2 * Hkv) * D), device=x.device, dtype=bf16)
+    ws = gemm_workspace(x.device)
+    Tmax = k_cache.shape[2]
+    with _Timed(("gemm_w4a16", n_tok, (H + 2 * Hkv) * D, K, EPI_BIAS | 32)):
+        check(
+            lib.af3_gemm_qkv_rope_w4a16(stream_ptr(), ptr(x), x.stride(0), ptr(w_packed), w_packed.stride(0), ptr(w_scale),
+                                        w_scale.stride(0), ptr(bias), ptr(out), out.stride(0), n_tok, K, H, Hkv, D, ptr(rope_cs),
+                                        ptr(k_cache), ptr(v_cache), Tmax, ptr(pos_dev), ptr(ws), ws.numel()),
+            "af3_gemm_qkv_rope_w4a16",
+        )
+    _count(1)
+    return out
+
+
+def dequant_w4a16(w_packed, w_scale, out=None):
+    """Wd = bf16(q * s) as bf16 [N, K] from w_packed int32 [N, K / 8] and w_scale bf16 [N, K / 128].  out: a bf16 buffer of at
+    least N * K elements whose first N * K hold the result (a scratch reused across projections); the [N, K] view is returned."""
+    lib = _lib.load()
+    _req(w_packed, torch.int32, "w_packed"), _req(w_scale, bf16, "w_scale")
+    N, words = w_packed.shape
+    K = words * 8
+    if K % 128 or tuple(w_scale.shape) != (N, K // 128):
+        raise _lib.AF3Error(f"dequant_w4a16: w_packed {tuple(w_packed.shape)} and w_scale {tuple(w_scale.shape)} do not match")
+    if out is None:
+        out = torch.empty((N * K,), device=w_packed.device, dtype=bf16)
+    _req(out, bf16, "out")
+    if out.numel() < N * K:
+        raise _lib.AF3Error(f"dequant_w4a16: out holds {out.numel()} elements, {N * K} needed")
+    wd = out.view(-1)[: N * K].view(N, K)
+    with _Timed(("dequant_w4a16", N, K, 0, 0)):
+        check(lib.af3_dequant_w4a16(stream_ptr(), ptr(w_packed), w_packed.stride(0), ptr(w_scale), w_scale.stride(0), ptr(wd), N, K),
+              "af3_dequant_w4a16")
+    _count(1)
+    return wd
+
+
 # ----------------------------------------------------------------------------------------------- log-mel
 class LogMelTables:
     """Constant tables of the log-mel kernel, built exactly as the reference builds its constants."""

@@ -105,6 +105,32 @@ int af3_gemm_qkv_rope_fp8(void* stream, const void* x, int ldx, const float* x_s
                           const float* rope_cs, void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace,
                           size_t workspace_bytes);
 
+/* ---- W4A16 decoder projections: group-wise int4 weights, bf16 activations, fp32 accumulation.  Additive (ABI v4).
+ *
+ * Format of a weight W [N, K] (nn.Linear layout), K and N multiples of 128.  Group g of row n is W[n, 128g : 128g + 128];
+ * its scale is s[n, g] = bf16(amax / 7.5) with amax = max |W| over the group in fp32 (IEEE division, round to nearest
+ * even), s = 1 when amax == 0; q[n, k] = clamp(round_half_even(W[n, k] / s[n, k / 128]), -8, 7) in fp32.
+ *   w_packed int32 [N, K/8] (pitch ldw words, ldw % 4 == 0): bits 4j .. 4j+3 of word i of row n hold q[n, 8i + j] + 8;
+ *   w_scale  bf16  [N, K/128] (pitch ld_scale elements).
+ * Every kernel computes with Wd[n, k] = bf16(q[n, k] * s[n, k / 128]) (one bf16 multiply, round to nearest even).
+ *
+ * out[t, n] = epi( sum_k x[t, k] Wd[n, k] ), x bf16 [n_tok, K] (pitch ldx), for n_tok <= 64 only (returns an error above
+ * that: use af3_dequant_w4a16 and af3_gemm_bf16).  flags: 0, AF3_EPI_BIAS, AF3_EPI_RESID (out may alias resid) or
+ * AF3_EPI_SWIGLU | AF3_EPI_SWIGLU_CONCAT on the [gate (n_feat rows); up (n_feat rows)] concatenation.  The workspace is that
+ * of af3_gemm_bf16_ws (split-K).  Without a workspace the result equals af3_gemm_bf16 on Wd bit for bit (same products,
+ * same k order, same epilogue). */
+int af3_gemm_w4a16(void* stream, const void* x, int ldx, const void* w_packed, int ldw, const void* w_scale, int ld_scale, void* out,
+                   int ldo, int n_tok, int n_feat, int K, int flags, const void* bias, const void* resid, int ld_res, void* workspace,
+                   size_t workspace_bytes);
+
+/* W4A16 counterpart of af3_gemm_qkv_rope: same outputs and cache writes at *pos_dev, n_tok <= 64. */
+int af3_gemm_qkv_rope_w4a16(void* stream, const void* x, int ldx, const void* w_packed, int ldw, const void* w_scale, int ld_scale,
+                            const void* bias, void* q_out, int ldo, int n_tok, int K, int H, int Hkv, int D, const float* rope_cs,
+                            void* k_cache, void* v_cache, int Tmax, const int* pos_dev, void* workspace, size_t workspace_bytes);
+
+/* Wd as bf16 [rows, K] (pitch K, out 16-byte aligned), for the GEMMs of more than 64 tokens. */
+int af3_dequant_w4a16(void* stream, const void* w_packed, int ldw, const void* w_scale, int ld_scale, void* out, int rows, int K);
+
 /* ---- Teacher-forced loss: the LM head with the cross-entropy of [O] loss/loss_utils.py ForCausalLMLoss ->
  * fixed_cross_entropy fused into its epilogue, without materialising the [n_tok, V] logits.  Additive (ABI v4).
  *
